@@ -118,6 +118,27 @@ typedef struct vpt_predictor_info {
 } vpt_predictor_info;
 int vpt_predictor_get_info(const vpt_predictor* predictor, vpt_predictor_info* out);
 
+/* The scoring kernel a batch of this predictor runs, the template variant of it and its tile geometry.  with_states != 0:
+ * a batch that asks for pattern-id states (char_states_out / type_states_out).  Works on host-only handles too. */
+typedef struct vpt_kernel_plan {
+    int32_t kernel;             /* 1 k_fused, 2 k_tile_fast, 3 k_score_fast, 4 k_score_general */
+    int32_t seeds_smem;         /* k_fused, k_tile_fast: perfect-hash seed bytes staged in shared memory */
+    int32_t common_shape;       /* k_fused: char window 3 + type window 3 with split tables */
+    int32_t deep;               /* k_fused: 0 patterns <= 3 chars, 1 longer ones, 2 also rows outside the inline window */
+    int32_t states;             /* k_fused: pattern-id states are written */
+    int32_t r0_fixed;           /* k_tile_fast: inline window start -3 compiled in */
+    int32_t general;            /* k_tile_fast: general rows */
+    int32_t split3;             /* k_tile_fast: type window 3 with split tables */
+    int32_t overflow;           /* k_tile_fast: long dictionary rows */
+    int32_t text_cap;           /* bytes of text a tile stages (0: no tiles, one warp per sentence) */
+    int32_t slot_cap;           /* character + separator slots per tile */
+    int32_t gap;                /* separator slots in front of every sentence of a tile */
+    int32_t lag;                /* k_fused: slots between a boundary's slot and the slot that finishes it */
+    int32_t sub_blocks;         /* independent 256-thread sub-blocks per CTA */
+    int32_t group;              /* sentences per group */
+} vpt_kernel_plan;
+int vpt_predictor_kernel_plan(const vpt_predictor* predictor, int with_states, vpt_kernel_plan* out);
+
 /* Flat device model: serialise on one rank, broadcast as bytes (NCCL), rebuild on the others.
  * (Replaces `Predictor::serialize_to_vec` / `deserialize_from_slice_unchecked`, predictor.rs:640-664, whose
  * daachorse-private layout is not reproducible; the blob format is this library's own.)

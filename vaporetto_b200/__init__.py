@@ -59,6 +59,14 @@ class _Info(C.Structure):
                 ("blob_bytes", C.c_uint64), ("kernel_launches_per_batch", C.c_int32)]
 
 
+class _KernelPlan(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("kernel", "seeds_smem", "common_shape", "deep", "states", "r0_fixed", "general",
+                                         "split3", "overflow", "text_cap", "slot_cap", "gap", "lag", "sub_blocks", "group")]
+
+
+KERNEL_NAMES = {1: "k_fused", 2: "k_tile_fast", 3: "k_score_fast", 4: "k_score_general"}
+
+
 # every symbol include/vaporetto_b200.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 ABI = [
@@ -78,6 +86,7 @@ ABI = [
     ("vpt_predictor_new", C.c_int, [_P, C.c_int, C.c_int, C.POINTER(_P)]),
     ("vpt_predictor_free", None, [_P]),
     ("vpt_predictor_get_info", C.c_int, [_P, C.POINTER(_Info)]),
+    ("vpt_predictor_kernel_plan", C.c_int, [_P, C.c_int, C.POINTER(_KernelPlan)]),
     ("vpt_blob_build", C.c_int, [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_uint64)]),
     ("vpt_blob_free", None, [_P]),
     ("vpt_predictor_blob_size", C.c_uint64, [_P]),
@@ -313,6 +322,16 @@ class Predictor:
         self.info = {k: getattr(info, k) for k, _ in _Info._fields_}
         self.n_tags = info.n_tags
         self.predict_tags = bool(info.predict_tags)
+
+    def kernel_plan(self, states: bool = False) -> dict:
+        """The scoring kernel a batch runs (`kernel`: k_fused, k_tile_fast, k_score_fast or k_score_general), its
+        template switches and its tile geometry (vpt_predictor_kernel_plan); `states`: a batch that asks for
+        pattern-id states."""
+        pl = _KernelPlan()
+        _check(lib().vpt_predictor_kernel_plan(self._h, int(states), C.byref(pl)))
+        out = {k: getattr(pl, k) for k, _ in _KernelPlan._fields_}
+        out["kernel"] = KERNEL_NAMES[pl.kernel]
+        return out
 
     def export_blob(self) -> np.ndarray:
         n = lib().vpt_predictor_blob_size(self._h)

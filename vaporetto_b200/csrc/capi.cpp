@@ -18,6 +18,7 @@
 #include "builder.hpp"
 #include "common.hpp"
 #include "device_model.hpp"
+#include "kernel_plan.hpp"
 #include "model.hpp"
 #include "predictor_build.hpp"
 #include "grapheme.hpp"
@@ -183,6 +184,8 @@ void validate_blob_header(const BlobHeader& h, uint64_t len) {
     if (h.type_state3_off && !inside(h.type_state3_off, 4 * 512)) throw bad("type state table");
 }
 
+DevModel dev_model(const BlobHeader& h, const uint8_t* base);
+
 void upload(vpt_predictor& p) {
     if (p.device == -1) return;  // host-only handle (tag prediction / Sentence helpers); cannot score
     int ndev = 0;
@@ -194,20 +197,24 @@ void upload(vpt_predictor& p) {
     cuda_check(cudaSetDevice(p.device), "cudaSetDevice");
     cuda_check(cudaMalloc(&p.d_blob, align_up(p.blob.size(), 256)), "cudaMalloc(model)");
     cuda_check(cudaMemcpy(p.d_blob, p.blob.data(), p.blob.size(), cudaMemcpyHostToDevice), "cudaMemcpy(model)");
-    const uint8_t* base = static_cast<const uint8_t*>(p.d_blob);
-    const BlobHeader& h = p.hdr;
-    p.dm = DevModel();
-    p.dm.ct = dev_table(h.ct, base);
-    p.dm.tt = dev_table(h.tt, base);
-    p.dm.type_cache_window = h.type_cache_window;
-    p.dm.type_cache = h.type_cache_window ? reinterpret_cast<const int32_t*>(base + h.type_cache_off) : nullptr;
-    p.dm.type_a = h.type_a_off ? reinterpret_cast<const int32_t*>(base + h.type_a_off) : nullptr;
-    p.dm.type_b = h.type_b_off ? reinterpret_cast<const int32_t*>(base + h.type_b_off) : nullptr;
-    p.dm.type_state3 = h.type_state3_off ? reinterpret_cast<const uint32_t*>(base + h.type_state3_off) : nullptr;
-    p.dm.bias = h.bias;
-    p.dm.char_window = h.char_window;
-    p.dm.type_window = h.type_window;
-    p.dm.emit_states = h.emit_states;
+    p.dm = dev_model(p.hdr, static_cast<const uint8_t*>(p.d_blob));
+}
+
+// The device view of a blob at `base` (the device copy, or the host copy when only the shape matters: kernel_plan)
+DevModel dev_model(const BlobHeader& h, const uint8_t* base) {
+    DevModel dm;
+    dm.ct = dev_table(h.ct, base);
+    dm.tt = dev_table(h.tt, base);
+    dm.type_cache_window = h.type_cache_window;
+    dm.type_cache = h.type_cache_window ? reinterpret_cast<const int32_t*>(base + h.type_cache_off) : nullptr;
+    dm.type_a = h.type_a_off ? reinterpret_cast<const int32_t*>(base + h.type_a_off) : nullptr;
+    dm.type_b = h.type_b_off ? reinterpret_cast<const int32_t*>(base + h.type_b_off) : nullptr;
+    dm.type_state3 = h.type_state3_off ? reinterpret_cast<const uint32_t*>(base + h.type_state3_off) : nullptr;
+    dm.bias = h.bias;
+    dm.char_window = h.char_window;
+    dm.type_window = h.type_window;
+    dm.emit_states = h.emit_states;
+    return dm;
 }
 
 // Tag tables of a tag predictor: built on the host (tags_build.cpp), one device allocation.
@@ -537,6 +544,30 @@ int vpt_predictor_get_info(const vpt_predictor* p, vpt_predictor_info* o) {
     o->max_char_pattern_len = uint32_t(p->hdr.max_char_pattern_len);
     o->blob_bytes = p->blob.size();
     o->kernel_launches_per_batch = launches_per_batch(p->dm);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_predictor_kernel_plan(const vpt_predictor* p, int with_states, vpt_kernel_plan* o) {
+    VPT_API_BEGIN
+    if (!p || !o) throw Error(kInvalidArgument, "InvalidArgumentError: predictor/out: must not be NULL");
+    const KernelPlan pl = plan(p->d_blob ? p->dm : dev_model(p->hdr, p->blob.data()), with_states != 0);
+    memset(o, 0, sizeof *o);
+    o->kernel = pl.kernel;
+    o->seeds_smem = pl.seeds_smem;
+    o->common_shape = pl.common;
+    o->deep = pl.deep;
+    o->states = pl.states;
+    o->r0_fixed = pl.r0_fixed;
+    o->general = pl.general;
+    o->split3 = pl.split3;
+    o->overflow = pl.overflow;
+    o->text_cap = pl.text_cap;
+    o->slot_cap = pl.slot_cap;
+    o->gap = pl.gap;
+    o->lag = pl.lag;
+    o->sub_blocks = pl.sub_blocks;
+    o->group = pl.group;
     return kOk;
     VPT_API_END
 }

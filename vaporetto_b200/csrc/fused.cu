@@ -1,40 +1,22 @@
-// vaporetto_b200 — host side of k_fused (fused_kernel.cuh): model-shape checks and the dispatch to the kernel variants,
-// which are instantiated in fused_ss.cu / fused_sg.cu / fused_gs.cu / fused_gg.cu (one translation unit per
-// (seeds in shared memory, common shape) pair, so that they compile in parallel).
+// vaporetto_b200 — host side of k_fused (fused_kernel.cuh): the dispatch to the kernel variants plan() chooses
+// (kernel_plan.hpp), which are instantiated in fused_ss.cu / fused_sg.cu / fused_gs.cu / fused_gg.cu (one translation
+// unit per (seeds in shared memory, common shape) pair, so that they compile in parallel).
 #include <atomic>
 #include <algorithm>
 
 #include "device_model.hpp"
 #include "fused_launch.hpp"
+#include "kernel_plan.hpp"
 
 namespace vpt {
 
-static bool fused_inline_ok(const DevModel& m) { return (!m.ct.present || m.ct.fast) && !m.tt.present; }
-
-static int fused_gap(const DevModel& m) {
-    const int tw = std::max(2, m.type_cache_window - 1);
-    const int r0 = m.ct.present ? m.ct.r0 : 0;
-    return std::max(tw, std::max(-r0 - 1, r0 + kInlineWidth - 1));
-}
-
-static int fused_lag(const DevModel& m) {
-    const int r0 = m.ct.present ? m.ct.r0 : 0;
-    return std::max(std::max(-r0, m.type_cache_window), 1);
-}
-
-bool fused_ok(const DevModel& m) {
-    if (!fused_inline_ok(m)) return false;
-    const int r0 = m.ct.present ? m.ct.r0 : 0;
-    const int tw = m.type_cache_window;
-    if (r0 < -5 || r0 > 0 || tw < 0 || tw > 3) return false;
-    if (fused_gap(m) > 8) return false;
-    if (m.emit_states && m.ct.present && m.ct.max_depth == 0) return false;
-    return fused_lag(m) + std::max(tw, 1) <= 6;  // the packed type history holds t[p-5 .. p]
-}
+bool fused_ok(const DevModel& m) { return plan_detail::fused_shape_ok(m); }
 
 // One launch for the whole batch (plus the memset node that clears the look-back descriptors and the ticket).
 cudaError_t launch_fused(const DevModel& m, const BatchArgs& a, cudaStream_t stream) {
     if (a.n_sent == 0) return cudaSuccess;
+    const KernelPlan pl = plan(m, a.char_states != nullptr || a.type_states != nullptr);
+    if (pl.kernel != kPlanFused) return cudaErrorInvalidValue;  // (callers check fused_ok first)
     static std::atomic<int> sm_count[fused_detail::kMaxDevices] = {};  // (idempotent cache: every writer stores the same value)
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -53,18 +35,14 @@ cudaError_t launch_fused(const DevModel& m, const BatchArgs& a, cudaStream_t str
         if (e != cudaSuccess) return e;
     }
     StreamCfg cfg;
-    cfg.lag = fused_lag(m);
+    cfg.lag = pl.lag;
     cfg.r0 = m.ct.present ? m.ct.r0 : 0;
-    cfg.gap = fused_gap(m);
+    cfg.gap = pl.gap;
     cfg.tw = m.type_cache_window;
     cfg.norm = m.kytea_norm != 0;
-    const bool seeds_smem = m.ct.present && !m.ct.seed16 && m.ct.nbuckets <= uint32_t(fused_detail::kSeedCap);
-    // the usual shape: char window 3 (inline window starts at -3) + type window 3 with split tables
-    const bool common = m.type_a != nullptr && m.type_cache_window == 3 && m.ct.present && m.ct.r0 == -3 &&
-                        cfg.gap == fused_detail::kCommonGap;
     const int n_sm = sm_count[dev];
-    if (seeds_smem) return common ? fused_detail::launch_fused_group<true, true>(m, a, cfg, stream, dev, n_sm) : fused_detail::launch_fused_group<true, false>(m, a, cfg, stream, dev, n_sm);
-    return common ? fused_detail::launch_fused_group<false, true>(m, a, cfg, stream, dev, n_sm) : fused_detail::launch_fused_group<false, false>(m, a, cfg, stream, dev, n_sm);
+    if (pl.seeds_smem) return pl.common ? fused_detail::launch_fused_group<true, true>(pl, m, a, cfg, stream, dev, n_sm) : fused_detail::launch_fused_group<true, false>(pl, m, a, cfg, stream, dev, n_sm);
+    return pl.common ? fused_detail::launch_fused_group<false, true>(pl, m, a, cfg, stream, dev, n_sm) : fused_detail::launch_fused_group<false, false>(pl, m, a, cfg, stream, dev, n_sm);
 }
 
 }  // namespace vpt

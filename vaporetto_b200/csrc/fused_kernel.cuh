@@ -31,6 +31,7 @@
 #include <type_traits>
 
 #include "fused_launch.hpp"
+#include "kernel_plan.hpp"
 #include "kernels_common.cuh"
 #include "utf8_window.hpp"
 
@@ -112,6 +113,10 @@ struct FLayout {
     static_assert(kSubBlocks >= ((kOverflow && kSeedsSmem) ? 3 : 4),
                   "shared memory budget: four sub-blocks per SM (three with the overflow sums next to the seed table)");
     static_assert(int(sizeof(Rings)) <= 4 * kFSlotAlloc, "fallback ring aliases the slot array");
+    // what plan() reports (kernel_plan.hpp) is what this variant is built with
+    static_assert(kFTextCap == plan_detail::fused_text_cap(kSeedsSmem, kStates, kOverflow), "text buffer differs from the plan");
+    static_assert(kFSlotCap == plan_detail::fused_slot_cap(kSeedsSmem, kStates, kOverflow), "slot buffer differs from the plan");
+    static_assert(kSubBlocks == plan_detail::fused_sub_blocks(kSeedsSmem, kOverflow), "sub-blocks differ from the plan");
 };
 
 __device__ __forceinline__ void fsub_sync(int sub) {
@@ -991,16 +996,13 @@ cudaError_t launch_fused_t(const DevModel& m, const BatchArgs& a, const StreamCf
 }
 
 template <bool kSeeds, bool kCommon>
-cudaError_t launch_fused_group(const DevModel& m, const BatchArgs& a, const StreamCfg& cfg, cudaStream_t stream, int dev, int n_sm) {
-    // patterns longer than three symbols (dictionary words) need the backward walk; their rows may stick out of the window
-    const int deep = !m.ct.present || m.ct.max_depth <= 3 ? 0 : (m.ct.has_overflow ? 2 : 1);
-    const bool states = a.char_states != nullptr || a.type_states != nullptr;
-    if (deep == 2) return states ? launch_fused_t<kSeeds, kCommon, 2, true>(m, a, cfg, stream, dev, n_sm)
-                                 : launch_fused_t<kSeeds, kCommon, 2, false>(m, a, cfg, stream, dev, n_sm);
-    if (deep == 1) return states ? launch_fused_t<kSeeds, kCommon, 1, true>(m, a, cfg, stream, dev, n_sm)
-                                 : launch_fused_t<kSeeds, kCommon, 1, false>(m, a, cfg, stream, dev, n_sm);
-    return states ? launch_fused_t<kSeeds, kCommon, 0, true>(m, a, cfg, stream, dev, n_sm)
-                  : launch_fused_t<kSeeds, kCommon, 0, false>(m, a, cfg, stream, dev, n_sm);
+cudaError_t launch_fused_group(const KernelPlan& pl, const DevModel& m, const BatchArgs& a, const StreamCfg& cfg, cudaStream_t stream, int dev, int n_sm) {
+    if (pl.deep == 2) return pl.states ? launch_fused_t<kSeeds, kCommon, 2, true>(m, a, cfg, stream, dev, n_sm)
+                                       : launch_fused_t<kSeeds, kCommon, 2, false>(m, a, cfg, stream, dev, n_sm);
+    if (pl.deep == 1) return pl.states ? launch_fused_t<kSeeds, kCommon, 1, true>(m, a, cfg, stream, dev, n_sm)
+                                       : launch_fused_t<kSeeds, kCommon, 1, false>(m, a, cfg, stream, dev, n_sm);
+    return pl.states ? launch_fused_t<kSeeds, kCommon, 0, true>(m, a, cfg, stream, dev, n_sm)
+                     : launch_fused_t<kSeeds, kCommon, 0, false>(m, a, cfg, stream, dev, n_sm);
 }
 
 }  // namespace fused_detail

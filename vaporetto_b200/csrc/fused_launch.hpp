@@ -14,6 +14,8 @@ struct StreamCfg {
     bool norm;
 };
 
+struct KernelPlan;  // kernel_plan.hpp
+
 namespace fused_detail {
 
 constexpr int kSeedCap = 37632;   // seed bytes the kernel keeps in shared memory
@@ -25,12 +27,12 @@ constexpr int kMaxDevices = 64;
 constexpr int kCommonGap = 2;     // separator slots between sentences for the common shape (char window 3, type window 3)
 
 template <bool kSeeds, bool kCommon>
-cudaError_t launch_fused_group(const DevModel& m, const BatchArgs& a, const StreamCfg& cfg, cudaStream_t stream, int dev, int n_sm);
+cudaError_t launch_fused_group(const KernelPlan& pl, const DevModel& m, const BatchArgs& a, const StreamCfg& cfg, cudaStream_t stream, int dev, int n_sm);
 
-extern template cudaError_t launch_fused_group<true, true>(const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
-extern template cudaError_t launch_fused_group<true, false>(const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
-extern template cudaError_t launch_fused_group<false, true>(const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
-extern template cudaError_t launch_fused_group<false, false>(const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
+extern template cudaError_t launch_fused_group<true, true>(const KernelPlan&, const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
+extern template cudaError_t launch_fused_group<true, false>(const KernelPlan&, const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
+extern template cudaError_t launch_fused_group<false, true>(const KernelPlan&, const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
+extern template cudaError_t launch_fused_group<false, false>(const KernelPlan&, const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
 
 }  // namespace fused_detail
 

@@ -3,6 +3,6 @@
 
 namespace vpt {
 namespace fused_detail {
-template cudaError_t launch_fused_group<true, false>(const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
+template cudaError_t launch_fused_group<true, false>(const KernelPlan&, const DevModel&, const BatchArgs&, const StreamCfg&, cudaStream_t, int, int);
 }  // namespace fused_detail
 }  // namespace vpt

@@ -27,6 +27,7 @@
 #include <cuda_runtime.h>
 
 #include "device_model.hpp"
+#include "kernel_plan.hpp"
 #include "keys.hpp"
 #include "textnorm.hpp"
 
@@ -395,6 +396,9 @@ static_assert(4 * kSlotCap <= kTextCap, "sc aliases the text buffer");
 static_assert(2 * (kSlotCap / 32) * 8 * 4 <= 2 * kSlotCap, "spill arrays alias the position buffer");
 static_assert(int(sizeof(Rings)) * (kSubThreads / 32) <= kOffPos, "fallback rings alias text+cp");
 static_assert(kTileSmem <= 227 * 1024, "shared memory budget");
+// what plan() reports (kernel_plan.hpp) is what the kernel is built with
+static_assert(kTextCap == plan_detail::kTileTextCap && kSlotCap == plan_detail::kTileSlotCap, "tile buffers differ from the plan");
+static_assert(kSubBlocks == plan_detail::kTileSubBlocks && kSeedCap == fused_detail::kSeedCap, "tile geometry differs from the plan");
 
 __device__ __forceinline__ void sub_sync(int sub) {
     asm volatile("bar.sync %0, %1;" ::"r"(sub + 1), "r"(kSubThreads) : "memory");
@@ -884,29 +888,10 @@ cudaError_t launch_count(const BatchArgs& a, cudaStream_t stream) {
     return e != cudaSuccess ? e : launch_scan_only(a, stream);
 }
 
-static bool use_fast(const DevModel& m) {
-    return (!m.ct.present || m.ct.fast) && !m.tt.present;
-}
-
-// separator slots between sentences of a tile so that neither the weight-row gather (window
-// [r0, r0+6)) nor the type window can reach a neighbouring sentence (general tables clip rows per sentence)
-static int tile_gap(const DevModel& m) {
-    const int tw = std::max(2, m.type_cache_window - 1);
-    if (!use_fast(m)) return tw;
-    const int r0 = m.ct.present ? m.ct.r0 : 0;
-    return std::max(tw, std::max(-r0 - 1, r0 + kInlineWidth - 1));
-}
-
-static bool tile_fast_ok(const DevModel& m) {
-    if (!use_fast(m)) return false;
-    const int r0 = m.ct.present ? m.ct.r0 : 0;
-    return r0 >= -8 && r0 <= 2 && tile_gap(m) <= 8 && m.type_cache_window <= 3;
-}
-
 constexpr int kMaxDevices = 64;
 
 template <bool kSeeds, int kR0, bool kGeneral, bool kSplit3, bool kOverflow>
-static cudaError_t launch_tile_t(const DevModel& m, const BatchArgs& a, cudaStream_t stream, int dev, int n_sm) {
+static cudaError_t launch_tile_t(const KernelPlan& pl, const DevModel& m, const BatchArgs& a, cudaStream_t stream, int dev, int n_sm) {
     static std::atomic<bool> attr_set[kMaxDevices] = {};  // the opt-in shared memory size is a per-device function attribute
     if (!attr_set[dev]) {
         cudaError_t e = cudaFuncSetAttribute(k_tile_fast<kSeeds, kR0, kGeneral, kSplit3, kOverflow>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem);
@@ -915,18 +900,17 @@ static cudaError_t launch_tile_t(const DevModel& m, const BatchArgs& a, cudaStre
     }
     const uint64_t ngroups = (a.n_sent + kGroup - 1) / kGroup;
     const unsigned grid = unsigned(std::min<uint64_t>(uint64_t(n_sm), (ngroups + kSubBlocks - 1) / kSubBlocks));
-    k_tile_fast<kSeeds, kR0, kGeneral, kSplit3, kOverflow><<<grid, kTileThreads, kTileSmem, stream>>>(m, a, tile_gap(m));
+    k_tile_fast<kSeeds, kR0, kGeneral, kSplit3, kOverflow><<<grid, kTileThreads, kTileSmem, stream>>>(m, a, pl.gap);
     return cudaGetLastError();
 }
 
 template <bool kSeeds, int kR0, bool kGeneral>
-static cudaError_t launch_tile(const DevModel& m, const BatchArgs& a, cudaStream_t stream, int dev, int n_sm) {
-    const bool split3 = m.type_a != nullptr && m.type_cache_window == 3;
-    if (!kGeneral && m.ct.present && m.ct.has_overflow)
-        return split3 ? launch_tile_t<kSeeds, kR0, false, true, true>(m, a, stream, dev, n_sm)
-                      : launch_tile_t<kSeeds, kR0, false, false, true>(m, a, stream, dev, n_sm);
-    return split3 ? launch_tile_t<kSeeds, kR0, kGeneral, true, false>(m, a, stream, dev, n_sm)
-                  : launch_tile_t<kSeeds, kR0, kGeneral, false, false>(m, a, stream, dev, n_sm);
+static cudaError_t launch_tile(const KernelPlan& pl, const DevModel& m, const BatchArgs& a, cudaStream_t stream, int dev, int n_sm) {
+    if (pl.overflow)
+        return pl.split3 ? launch_tile_t<kSeeds, kR0, false, true, true>(pl, m, a, stream, dev, n_sm)
+                         : launch_tile_t<kSeeds, kR0, false, false, true>(pl, m, a, stream, dev, n_sm);
+    return pl.split3 ? launch_tile_t<kSeeds, kR0, kGeneral, true, false>(pl, m, a, stream, dev, n_sm)
+                     : launch_tile_t<kSeeds, kR0, kGeneral, false, false>(pl, m, a, stream, dev, n_sm);
 }
 
 cudaError_t launch_batch(const DevModel& m, const BatchArgs& a, cudaStream_t stream) {
@@ -937,41 +921,31 @@ cudaError_t launch_batch(const DevModel& m, const BatchArgs& a, cudaStream_t str
 
 cudaError_t launch_score(const DevModel& m, const BatchArgs& a, cudaStream_t stream) {
     if (a.n_sent == 0) return cudaSuccess;
-    if (fused_ok(m)) return launch_fused(m, a, stream);  // self-contained: does not need the count pass
-    static std::atomic<int> sm_count[kMaxDevices] = {};  // (idempotent cache: every writer stores the same value)
-    int dev = 0;
-    cudaError_t e0 = cudaGetDevice(&dev);
-    if (e0 != cudaSuccess) return e0;
-    if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
-    if (sm_count[dev] == 0) {
-        int v = 0;
-        e0 = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    const KernelPlan pl = plan(m, a.char_states != nullptr || a.type_states != nullptr);
+    if (pl.kernel == kPlanFused) return launch_fused(m, a, stream);  // self-contained: does not need the count pass
+    if (pl.kernel == kPlanTileFast) {
+        static std::atomic<int> sm_count[kMaxDevices] = {};  // (idempotent cache: every writer stores the same value)
+        int dev = 0;
+        cudaError_t e0 = cudaGetDevice(&dev);
         if (e0 != cudaSuccess) return e0;
-        sm_count[dev] = v;
-    }
-    const int n_sm = sm_count[dev];
-    const bool seeds_smem = m.ct.present && !m.ct.seed16 && m.ct.nbuckets <= uint32_t(kSeedCap);
-    if (tile_fast_ok(m)) {
-        const bool r3 = m.ct.present && m.ct.r0 == -3;
-        if (seeds_smem && r3) return launch_tile<true, -3, false>(m, a, stream, dev, n_sm);
-        if (seeds_smem) return launch_tile<true, kRuntimeR0, false>(m, a, stream, dev, n_sm);
-        if (r3) return launch_tile<false, -3, false>(m, a, stream, dev, n_sm);
-        return launch_tile<false, kRuntimeR0, false>(m, a, stream, dev, n_sm);
-    }
-    if (use_fast(m)) {  // inline rows with an unusual window: one warp per sentence
-        const uint64_t nblocks = (a.n_sent + kWarpsPerBlock - 1) / kWarpsPerBlock;
-        k_score_fast<<<unsigned(nblocks), kWarpsPerBlock * 32, 0, stream>>>(m, a);
-        return cudaGetLastError();
-    }
-    // general tables through the tile kernel pay off for shallow pattern sets (n-gram models with tags); deep
-    // dictionaries (long rows, backward walks, seed array too large for shared memory) are faster one warp per
-    // sentence
-    if (m.type_cache_window <= 3 && m.ct.max_depth <= 3 && m.tt.max_depth <= 4) {
-        if (seeds_smem) return launch_tile<true, kRuntimeR0, true>(m, a, stream, dev, n_sm);
-        return launch_tile<false, kRuntimeR0, true>(m, a, stream, dev, n_sm);
+        if (dev < 0 || dev >= kMaxDevices) return cudaErrorInvalidDevice;
+        if (sm_count[dev] == 0) {
+            int v = 0;
+            e0 = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+            if (e0 != cudaSuccess) return e0;
+            sm_count[dev] = v;
+        }
+        const int n_sm = sm_count[dev];
+        if (pl.general) return pl.seeds_smem ? launch_tile<true, kRuntimeR0, true>(pl, m, a, stream, dev, n_sm)
+                                             : launch_tile<false, kRuntimeR0, true>(pl, m, a, stream, dev, n_sm);
+        if (pl.seeds_smem && pl.r0_fixed) return launch_tile<true, -3, false>(pl, m, a, stream, dev, n_sm);
+        if (pl.seeds_smem) return launch_tile<true, kRuntimeR0, false>(pl, m, a, stream, dev, n_sm);
+        if (pl.r0_fixed) return launch_tile<false, -3, false>(pl, m, a, stream, dev, n_sm);
+        return launch_tile<false, kRuntimeR0, false>(pl, m, a, stream, dev, n_sm);
     }
     const uint64_t nblocks = (a.n_sent + kWarpsPerBlock - 1) / kWarpsPerBlock;
-    k_score_general<<<unsigned(nblocks), kWarpsPerBlock * 32, 0, stream>>>(m, a);
+    if (pl.kernel == kPlanScoreFast) k_score_fast<<<unsigned(nblocks), kWarpsPerBlock * 32, 0, stream>>>(m, a);
+    else k_score_general<<<unsigned(nblocks), kWarpsPerBlock * 32, 0, stream>>>(m, a);
     return cudaGetLastError();
 }
 
@@ -979,6 +953,9 @@ int launches_per_batch(const DevModel& m) { return fused_ok(m) ? 1 : 3; }
 
 // The paths that accumulate into the score array itself (general rows, overflow rows of long sentences) need
 // it; the inline-row tile kernel keeps the sums in shared memory and can skip the score stores.
-bool scores_optional(const DevModel& m) { return (fused_ok(m) || tile_fast_ok(m)) && !m.ct.has_overflow; }
+bool scores_optional(const DevModel& m) {
+    const KernelPlan pl = plan(m, false);
+    return (pl.kernel == kPlanFused || (pl.kernel == kPlanTileFast && !pl.general)) && !m.ct.has_overflow;
+}
 
 }  // namespace vpt
