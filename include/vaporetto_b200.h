@@ -351,6 +351,37 @@ int vpt_tokenize_lines(const vpt_predictor* predictor, const uint8_t* utf8, size
 int vpt_tokenize_lines_tags(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes, int no_norm,
                             uint32_t wsconst_types, uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
 
+/* The reference's `evaluate` command (evaluate/src/main.rs:69-195) over a buffer holding a gold corpus in the tokenized
+ * format (`まぁ/名詞/マー 社長/名詞/シャチョー ...`, one sentence per line).  Lines are split as in vpt_tokenize_lines;
+ * an empty line is skipped.  Every other line is parsed by `Sentence::from_tokenized` (sentence.rs:285-467) for the
+ * gold boundaries and tags, predicted like the `predict` CLI (KyteaFullwidthFilter unless `no_norm`, the
+ * `wsconst_types` post-filters, and with `predict_tags` fill_tags) and compared with the gold:
+ *   - char metric (main.rs:121-147): tp, tn, fp, fn over all character boundaries;
+ *   - word metric (main.rs:149-191, Nagata 1994): n_sys / n_ref are the system / gold tokens, n_cor the tokens both
+ *     have at the same span with equal tags.  Tags compare as the reference's Vec<Option<String>>: with no_norm and no
+ *     tag prediction the sentence keeps the gold tags (always equal); normalised without tag prediction it has none
+ *     (equal only on lines without a tag field); with tag prediction and a model with k > 0 tag slots, a token is equal
+ *     where its line has exactly k gold tag fields on some token and every slot matches (a predictor with k == 0 keeps
+ *     the sentence's tags, predictor.rs:553).
+ * Parsing, prediction and both metrics run on the device; only the totals (and the optional per-line counts) come back.
+ * Errors stop the whole call, as they stop the CLI, and name the 0-based line (every line counts, empty ones too):
+ * the lowest bad line's first violation, in the order the reference's character loop meets them, returns
+ * VPT_INVALID_ARGUMENT "InvalidArgumentError: tokenized_text: <reason>"; a line that is not valid UTF-8 returns
+ * VPT_IO_ERROR ("stream did not contain valid UTF-8").  Two documented differences: a line holding a lone '\' has no
+ * character and is the "must contain at least one character" error (the reference divides by zero,
+ * sentence.rs:450), and the counts are 64-bit (the reference's i32 counters wrap beyond 2^31).
+ * `predict_tags` and `wsconst_types` are checked as in vpt_tokenize_lines_tags.  `line_counts` (nullable) receives
+ * tp, tn, fp, fn, n_sys, n_ref, n_cor of every input line (zeros for empty lines), `line_capacity` rows of 7; a
+ * buffer with fewer rows than lines returns VPT_INVALID_ARGUMENT after the totals are filled in. */
+typedef struct vpt_eval_counts {
+    uint64_t n_lines, n_sentences;       /* input lines; non-empty lines evaluated */
+    uint64_t tp, tn, fp, fn;             /* --metric char  (evaluate/src/main.rs:121-147) */
+    uint64_t n_sys, n_ref, n_cor;        /* --metric word  (:149-191, Nagata 1994) */
+} vpt_eval_counts;
+int vpt_evaluate_lines(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes, int no_norm,
+                       uint32_t wsconst_types, int predict_tags, vpt_eval_counts* out,
+                       uint32_t* line_counts /* nullable, [n_lines * 7] */, uint64_t line_capacity);
+
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */
 uint32_t vpt_kytea_fullwidth(uint32_t code_point);

@@ -142,6 +142,24 @@ public:
         return out;
     }
 
+    /// The reference's `evaluate` command (evaluate/src/main.rs:69-195; `vpt_evaluate_lines`) over a gold corpus in
+    /// the tokenized format: the counts of both metrics.  `line_counts` (optional) receives tp, tn, fp, fn, n_sys,
+    /// n_ref, n_cor of every input line.
+    vpt_eval_counts evaluate_lines(const std::string& text, bool no_norm = false, uint32_t wsconst_types = 0,
+                                   bool predict_tags = false, std::vector<uint32_t>* line_counts = nullptr) const {
+        vpt_eval_counts c{};
+        uint64_t n_lines = 0;
+        if (line_counts) {
+            for (char ch : text) n_lines += ch == '\n';
+            if (!text.empty() && text.back() != '\n') ++n_lines;
+            line_counts->assign(size_t(n_lines) * 7, 0);
+        }
+        detail::check(vpt_evaluate_lines(h_, reinterpret_cast<const uint8_t*>(text.data()), text.size(), no_norm ? 1 : 0,
+                                         wsconst_types, predict_tags ? 1 : 0, &c,
+                                         line_counts ? line_counts->data() : nullptr, n_lines));
+        return c;
+    }
+
     /// Result of `predict_batch_compact`: see `vpt_predict_batch_compact` (include/vaporetto_b200.h).
     struct CompactResult {
         std::vector<uint32_t> boundary_bits;   // the batch's boundaries, one bit each

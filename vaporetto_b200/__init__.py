@@ -119,6 +119,7 @@ ABI = [
     ("vpt_unpack_boundaries", C.c_int, [_P, C.c_uint64, C.c_uint64, _P]),
     ("vpt_tokenize_lines_tags", C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, C.c_size_t,
                                           C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("vpt_evaluate_lines", C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, _P, _P, C.c_uint64]),
 ]
 
 _lib = None
@@ -452,11 +453,7 @@ class Predictor:
         out as space-separated tokens on the device; `wsconst`: letters of the CLI's --wsconst options ("D", "DR", ...:
         KyteaWsConstFilter; "G": ConcatGraphemeClustersFilter); `predict_tags`: the CLI's --predict-tags
         (vpt_tokenize_lines_tags).  Returns (uint8 view of the output lines, number of lines)."""
-        mask = 0
-        for ch in wsconst:
-            if ch not in "DRHTKOG":
-                raise VaporettoError(2, "InvalidArgumentError: wsconst: one of D, R, H, T, K, O, G")
-            mask |= 1 << ("DRHTKOG".index(ch) + 1)
+        mask = _wsconst_mask(wsconst)
         t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
         if out is None:
             out = np.empty((3 + (16 if predict_tags else 0)) * t.size + int(np.count_nonzero(t == 10)) + 16, np.uint8)
@@ -471,6 +468,43 @@ class Predictor:
             break
         _check(rc)
         return out[: n.value], int(nl.value)
+
+
+    def evaluate_lines(self, data, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
+                       per_line: bool = False):
+        """The reference's `evaluate` command (evaluate/src/main.rs:69-195, vpt_evaluate_lines) over a buffer holding a
+        gold corpus in the tokenized format: every non-empty line is parsed (Sentence::from_tokenized), predicted as
+        tokenize_lines predicts it (same `no_norm`, `wsconst`, `predict_tags`) and compared with its gold boundaries
+        and tags, all on the device.  Returns a dict of the counts (n_lines, n_sentences, tp, tn, fp, fn for
+        --metric char; n_sys, n_ref, n_cor for --metric word) and, with `per_line`, also a uint32 array
+        (n_lines, 7) of tp, tn, fp, fn, n_sys, n_ref, n_cor per input line.  A bad gold line raises VaporettoError
+        (InvalidArgument, or IOError for invalid UTF-8) naming the first such line."""
+        mask = _wsconst_mask(wsconst)
+        t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
+        counts = _EvalCounts()
+        lc = None
+        if per_line:
+            n_lines = int(np.count_nonzero(t == 10)) + (1 if t.size and t[-1] != 10 else 0)
+            lc = np.zeros((n_lines, 7), np.uint32)
+        _check(lib().vpt_evaluate_lines(self._h, t.ctypes.data, t.size, int(no_norm), mask, int(predict_tags),
+                                        C.byref(counts), _ptr(lc), 0 if lc is None else lc.shape[0]))
+        out = {name: int(getattr(counts, name)) for name, _ in _EvalCounts._fields_}
+        return (out, lc) if per_line else out
+
+
+class _EvalCounts(C.Structure):
+    _fields_ = [(name, C.c_uint64) for name in ("n_lines", "n_sentences", "tp", "tn", "fp", "fn", "n_sys", "n_ref",
+                                                "n_cor")]
+
+
+def _wsconst_mask(wsconst: str) -> int:
+    """The CLI's --wsconst letters as the C ABI's bit set (VPT_WSCONST_*)."""
+    mask = 0
+    for ch in wsconst:
+        if ch not in "DRHTKOG":
+            raise VaporettoError(2, "InvalidArgumentError: wsconst: one of D, R, H, T, K, O, G")
+        mask |= 1 << ("DRHTKOG".index(ch) + 1)
+    return mask
 
 
 class CompactResult:

@@ -71,15 +71,27 @@ struct Scratch {
     void* d_tokwork = nullptr; size_t tokwork_cap = 0;  // work list of the per-token tag kernels (TagArgs::tok_work)
     void* d_toklocal = nullptr; size_t toklocal_cap = 0;
     void* d_tokblk = nullptr; size_t tokblk_cap = 0;
+    // gold corpus and metrics (vpt_evaluate_lines)
+    void* d_gtext = nullptr; size_t gtext_cap = 0;
+    void* d_goff = nullptr; size_t goff_cap = 0;
+    void* d_gcoff = nullptr; size_t gcoff_cap = 0;
+    void* d_gbnd = nullptr; size_t gbnd_cap = 0;
+    void* d_gtag = nullptr; size_t gtag_cap = 0;
+    void* d_gw = nullptr; size_t gw_cap = 0;
+    void* d_lc = nullptr; size_t lc_cap = 0;
+    void* d_evtot = nullptr; size_t evtot_cap = 0;
+    uint64_t* h_eval = nullptr;    // pinned, kEvalTotals + 1 x u64: a chunk's totals and error key
     uint64_t* h_totals = nullptr;  // pinned, 8 x u64: boundaries, chars, lines, output bytes, tokens, first bit word
     uint32_t* h_side = nullptr; size_t side_cap = 0;  // pinned: first bit word of every chunk (vpt_predict_batch_compact)
     uint8_t* h_io = nullptr;       // pinned staging of the single-sentence call (vpt_predict), kSingleIoBytes
     void* d_io = nullptr;          // its device twin
     ~Scratch() {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
-                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk})
+                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk,
+                        d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
+        if (h_eval) cudaFreeHost(h_eval);
         if (h_io) cudaFreeHost(h_io);
         if (h_side) cudaFreeHost(h_side);
         if (d_io) cudaFree(d_io);
@@ -971,55 +983,35 @@ void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* utf8) {
     cuda_check(cudaEventRecord(ch.split, st), "cudaEventRecord");
 }
 
-// stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
-void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normalize, uint32_t wsconst, bool tags) {
+// Scores the sentences of `a` (text, offsets, trims, n_sent set; `nbytes` bounds their bytes), runs the --wsconst
+// post-filters and, with `tags`, predicts the tags of every token into per-token records (the post-filters ran first:
+// fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
+// records; its output fields are left to the caller.
+TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, bool normalize,
+                      uint32_t wsconst, bool tags) {
     cudaStream_t st = s.stream;
-    cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
-    const size_t n = size_t(s.h_totals[2]);
-    ch.n_lines = n;
-    if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
-    s.h_totals[3] = 0;
-    if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
+    const size_t n = size_t(a.n_sent);
     const WorkspaceLayout wl = workspace_layout(n);
-    const size_t ng = (n + kGroup - 1) / kGroup;
-    Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
     Scratch::ensure(s.d_ws, s.ws_cap, wl.total);
     Scratch::ensure(s.d_status, s.status_cap, 4 * n);
     Scratch::ensure(s.d_boff, s.boff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_bounds, s.bounds_cap, ch.nbytes + 4);
-    Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
-    // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
-    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
-    Scratch::ensure(s.d_out, s.out_cap, 3 * ch.nbytes + n + 4 + (tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0));
-    ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
-    ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
-    // the kernels overwrite d_out, which the previous chunk of this scratch may still be copying out
-    cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
-    if (pipeline_trace()) ch.tr.mark(1, st);
-    cuda_check(launch_split_write(ch.sp, st), "launch(split)");
-    BatchArgs a;
-    a.text = ch.sp.text;
-    a.offsets = ch.sp.offsets;
-    a.trims = ch.sp.trims;
-    a.n_sent = n;
+    Scratch::ensure(s.d_bounds, s.bounds_cap, nbytes + 4);
     bind_workspace(a, s.d_ws, n);
     a.status = static_cast<int32_t*>(s.d_status);
     a.bound_offsets = static_cast<uint64_t*>(s.d_boff);
-    // the tokenised text needs the boundaries only (every character is at least one byte: the chunk's bytes
-    // bound its boundaries)
+    // the callers need the boundaries only (every character is at least one byte: the bytes bound the boundaries)
     a.scores = nullptr;
     DevModel dm = p.dm;
     dm.kytea_norm = normalize ? 1 : 0;
     if (!scores_optional(dm)) {
-        Scratch::ensure(s.d_scores, s.scores_cap, 4 * ch.nbytes + 4);
+        Scratch::ensure(s.d_scores, s.scores_cap, 4 * nbytes + 4);
         a.scores = static_cast<int32_t*>(s.d_scores);
     }
     a.boundaries = static_cast<uint8_t*>(s.d_bounds);
     if (tags) {
         // tag prediction needs the pattern-id states and the character offsets of the sentences
-        Scratch::ensure(s.d_cst, s.cst_cap, 4 * ch.nbytes + 16);
-        Scratch::ensure(s.d_tst, s.tst_cap, 4 * ch.nbytes + 16);
+        Scratch::ensure(s.d_cst, s.cst_cap, 4 * nbytes + 16);
+        Scratch::ensure(s.d_tst, s.tst_cap, 4 * nbytes + 16);
         Scratch::ensure(s.d_coff, s.coff_cap, 8 * (n + 1));
         a.char_states = static_cast<uint32_t*>(s.d_cst);
         a.type_states = static_cast<uint32_t*>(s.d_tst);
@@ -1039,16 +1031,10 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normal
     t.n_chars = a.n_chars;
     t.boundaries = a.boundaries;
     t.bound_offsets = a.bound_offsets;
-    t.tok_state = static_cast<uint64_t*>(s.d_tokg);
-    t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
-    t.total = t.tok_state + ng + 1;
-    t.total_host = &s.h_totals[3];
-    t.out = static_cast<uint8_t*>(s.d_out);
     cuda_check(launch_wsconst(t, a.boundaries, wsconst, normalize, st), "launch(wsconst)");
     if (wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
     if (tags) {
-        // tokens per sentence and their prefix, then the tag prediction into per-token records (the post-filters ran:
-        // fill_tags sees the final boundaries, predict/src/main.rs:157-160)
+        // tokens per sentence and their prefix, then the tag prediction into per-token records
         CompactArgs k;
         k.n_sent = n;
         k.status = a.status;
@@ -1067,9 +1053,9 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normal
         k.tok_local = static_cast<uint32_t*>(s.d_toklocal);
         k.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
         cuda_check(launch_compact(k, st), "launch(compact)");
-        Scratch::ensure(s.d_tok, s.tok_cap, 4 * ch.nbytes + 16);
-        Scratch::ensure(s.d_cand, s.cand_cap, ch.nbytes * std::max<size_t>(p.n_tags, 1) + 16);
-        Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * ch.nbytes + 16);
+        Scratch::ensure(s.d_tok, s.tok_cap, 4 * nbytes + 16);
+        Scratch::ensure(s.d_cand, s.cand_cap, nbytes * std::max<size_t>(p.n_tags, 1) + 16);
+        Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * nbytes + 16);
         TagArgs g;
         g.text = a.text;
         g.offsets = a.offsets;
@@ -1085,8 +1071,8 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normal
         g.tok_ids = static_cast<int32_t*>(s.d_tok);
         g.tok_cands = static_cast<uint8_t*>(s.d_cand);
         g.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-        g.max_tokens = ch.nbytes;
-        Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * ch.nbytes + 32);
+        g.max_tokens = nbytes;
+        Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nbytes + 32);
         g.tok_work = static_cast<uint32_t*>(s.d_tokwork);
         g.norm = normalize ? 1 : 0;
         cuda_check(launch_tags(p.dt, g, st), "launch(tags)");
@@ -1099,6 +1085,42 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normal
         t.ts_ref = p.dt.ts_ref;
         t.ts_bytes = p.dt.ts_bytes;
     }
+    return t;
+}
+
+// stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
+void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normalize, uint32_t wsconst, bool tags) {
+    cudaStream_t st = s.stream;
+    cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
+    const size_t n = size_t(s.h_totals[2]);
+    ch.n_lines = n;
+    if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
+    s.h_totals[3] = 0;
+    if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
+    const size_t ng = (n + kGroup - 1) / kGroup;
+    Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
+    Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
+    // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
+    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
+    Scratch::ensure(s.d_out, s.out_cap, 3 * ch.nbytes + n + 4 + (tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0));
+    ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
+    ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
+    // the kernels overwrite d_out, which the previous chunk of this scratch may still be copying out
+    cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
+    if (pipeline_trace()) ch.tr.mark(1, st);
+    cuda_check(launch_split_write(ch.sp, st), "launch(split)");
+    BatchArgs a;
+    a.text = ch.sp.text;
+    a.offsets = ch.sp.offsets;
+    a.trims = ch.sp.trims;
+    a.n_sent = n;
+    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, normalize, wsconst, tags);
+    t.tok_state = static_cast<uint64_t*>(s.d_tokg);
+    t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
+    t.total = t.tok_state + ng + 1;
+    t.total_host = &s.h_totals[3];
+    t.out = static_cast<uint8_t*>(s.d_out);
     cuda_check(launch_tokenize(t, st), "launch(tok)");
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
@@ -1109,9 +1131,8 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normal
 uint32_t vpt_kytea_fullwidth(uint32_t code_point) { return kytea_fullwidth(code_point); }
 
 namespace {
-int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
-                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
-    VPT_API_BEGIN
+// The flags of the line loops (vpt_tokenize_lines*, vpt_evaluate_lines); returns whether tags are predicted on the device
+bool check_lines_flags(const vpt_predictor* p, uint32_t wsconst_types, bool tags) {
     require_device(p);
     if (tags) {
         if (!p->predict_tags || p->from_blob)
@@ -1120,16 +1141,14 @@ int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_by
             throw Error(kUnsupported, "this tag model exceeds the limits of the device path (tags.hpp); use vpt_fill_tags");
         if (p->n_tags == 0) tags = false;  // predictor.rs:553-555: nothing to predict
     }
-    if (out_len) *out_len = 0;
-    if (n_lines_out) *n_lines_out = 0;
     if (wsconst_types & ~0xFEu)
         throw Error(kInvalidArgument, "InvalidArgumentError: wsconst_types: bits 1..6 (Digit .. Other) and 7 (grapheme clusters) only");
-    if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
-    if (n_bytes == 0) return kOk;
-    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    return tags;
+}
 
-    // cut the buffer into chunks that end after a '\n' (memrchr from the nominal cut; a line longer than a
-    // chunk extends it to the line's end)
+// Cuts a buffer of lines into pipeline chunks that end after a '\n' (memrchr from the nominal cut; a line longer than a
+// chunk extends it to the line's end)
+std::vector<LineChunk> line_chunks(const uint8_t* utf8, size_t n_bytes) {
     const size_t big = chunk_bytes();
     const std::vector<size_t> sizes = ramp_schedule(n_bytes, big, big / 8, big / 8);
     std::vector<LineChunk> chunks;
@@ -1153,6 +1172,20 @@ int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_by
         chunks.push_back(ch);
         lo = hi;
     }
+    return chunks;
+}
+
+int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
+                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    VPT_API_BEGIN
+    tags = check_lines_flags(p, wsconst_types, tags);
+    if (out_len) *out_len = 0;
+    if (n_lines_out) *n_lines_out = 0;
+    if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
+    if (n_bytes == 0) return kOk;
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+
+    std::vector<LineChunk> chunks = line_chunks(utf8, n_bytes);
     const size_t nchunks = chunks.size();
     constexpr int kDepth = 4;
     std::unique_ptr<ScratchLease> lease[kDepth];
@@ -1220,6 +1253,191 @@ int vpt_tokenize_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_byt
 int vpt_tokenize_lines_tags(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
                             uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
     return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out);
+}
+
+namespace {
+
+// stage 1 of an evaluate chunk: line offsets, the gold parse, count + score + post-filters (+ tags) on the raw
+// sentences, the metrics; the chunk's totals and error key to pinned host memory, the per-line counts (if wanted) to
+// `line_counts` from row `line_lo`
+void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normalize, uint32_t wsconst, bool tags,
+                 int tag_mode, uint32_t* line_counts, uint64_t line_lo) {
+    cudaStream_t st = s.stream;
+    cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
+    const size_t n = size_t(s.h_totals[2]);
+    ch.n_lines = n;
+    if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
+    if (!s.h_eval) cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s.h_eval), 8 * (kEvalTotals + 1)), "cudaMallocHost");
+    if (n == 0) {
+        for (int i = 0; i < kEvalTotals; ++i) s.h_eval[i] = 0;
+        s.h_eval[kEvalTotals] = kGoldNoError;
+        cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
+        return;
+    }
+    const size_t ng = (n + kGroup - 1) / kGroup;
+    const size_t nb = ch.nbytes;  // bounds the surface bytes and characters of the chunk
+    Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
+    Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
+    Scratch::ensure(s.d_gtext, s.gtext_cap, nb + 64);
+    Scratch::ensure(s.d_goff, s.goff_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_gbnd, s.gbnd_cap, nb + 4);
+    Scratch::ensure(s.d_gw, s.gw_cap, 4 * n + 4);
+    Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
+    if (tag_mode == kTagsCompare) Scratch::ensure(s.d_gtag, s.gtag_cap, 4 * nb + 4);
+    if (line_counts) Scratch::ensure(s.d_lc, s.lc_cap, 28 * n + 4);
+    ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
+    ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
+    // the kernels overwrite d_lc, which the previous chunk of this scratch may still be copying out
+    cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
+    if (pipeline_trace()) ch.tr.mark(1, st);
+    cuda_check(launch_split_write(ch.sp, st), "launch(split)");
+    EvalArgs e;
+    e.text = ch.sp.text;
+    e.offsets = ch.sp.offsets;
+    e.trims = ch.sp.trims;
+    e.n_sent = n;
+    e.surface = static_cast<uint8_t*>(s.d_gtext);
+    e.surf_offsets = static_cast<uint64_t*>(s.d_goff);
+    e.char_offsets = static_cast<uint64_t*>(s.d_gcoff);
+    e.gold_bnd = static_cast<uint8_t*>(s.d_gbnd);
+    e.tag_pos = tag_mode == kTagsCompare ? static_cast<uint32_t*>(s.d_gtag) : nullptr;
+    e.width = static_cast<uint32_t*>(s.d_gw);
+    e.state = static_cast<uint64_t*>(s.d_tokg);
+    e.ticket = reinterpret_cast<uint32_t*>(e.state + ng);
+    e.totals = static_cast<uint64_t*>(s.d_evtot);
+    e.err = e.totals + kEvalTotals;
+    cuda_check(cudaMemsetAsync(e.totals, 0, 8 * kEvalTotals, st), "cudaMemset");
+    cuda_check(cudaMemsetAsync(e.err, 0xFF, 8, st), "cudaMemset");
+    cuda_check(launch_gold_parse(e, st), "launch(gold)");
+    BatchArgs a;
+    a.text = e.surface;
+    a.offsets = e.surf_offsets;
+    a.n_sent = n;
+    const TokArgs t = predict_lines(p, s, ch, a, nb, normalize, wsconst, tags);
+    e.status = t.status;
+    e.n_chars = t.n_chars;
+    e.boundaries = t.boundaries;
+    e.bound_offsets = t.bound_offsets;
+    e.tag_mode = tag_mode;
+    if (tag_mode == kTagsCompare) {
+        e.n_tags = t.n_tags;
+        e.tok_base = t.tok_base;
+        e.tok_ids = t.tok_ids;
+        e.tok_cands = t.tok_cands;
+        e.ts_slot = t.ts_slot;
+        e.ts_cand = t.ts_cand;
+        e.ts_ref = t.ts_ref;
+        e.ts_bytes = t.ts_bytes;
+    }
+    e.line_counts = line_counts ? static_cast<uint32_t*>(s.d_lc) : nullptr;
+    cuda_check(launch_eval(e, st), "launch(eval)");
+    cuda_check(cudaMemcpyAsync(s.h_eval, e.totals, 8 * (kEvalTotals + 1), cudaMemcpyDeviceToHost, st), "D2H(totals)");
+    if (pipeline_trace()) ch.tr.mark(2, st);
+    cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
+    if (line_counts) {
+        cuda_check(cudaEventRecord(s.ev_kernels, st), "cudaEventRecord");
+        cuda_check(cudaStreamWaitEvent(s.stream_out, s.ev_kernels, 0), "cudaStreamWaitEvent");
+        cuda_check(cudaMemcpyAsync(line_counts + 7 * line_lo, s.d_lc, 28 * n, cudaMemcpyDeviceToHost, s.stream_out), "D2H(counts)");
+        cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
+    }
+}
+
+const char* gold_error_text(uint32_t kind) {
+    switch (kind) {
+        case kGoldEmpty: return "must contain at least one character";
+        case kGoldStartWs: return "must not start with a whitespace";
+        case kGoldDoubleWs: return "must not contain consecutive whitespaces";
+        case kGoldSlash: return "a slash must follow a character";
+        case kGoldNul: return "must not contain NULL";
+        default: return "must not end with a whitespace";
+    }
+}
+
+}  // namespace
+
+int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
+                       int predict_tags, vpt_eval_counts* out, uint32_t* line_counts, uint64_t line_capacity) {
+    VPT_API_BEGIN
+    const bool tags = check_lines_flags(p, wsconst_types, predict_tags != 0);
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = vpt_eval_counts();
+    if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
+    if (n_bytes == 0) return kOk;
+    // main.rs:110-120 with predictor.rs:553: the system keeps the gold tags (--no-norm) or has none, unless tags are
+    // predicted with a model that has tag slots
+    const int tag_mode = tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty;
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+
+    std::vector<LineChunk> chunks = line_chunks(utf8, n_bytes);
+    const size_t nchunks = chunks.size();
+    constexpr int kDepth = 4;
+    std::unique_ptr<ScratchLease> lease[kDepth];
+    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
+    struct EventGuard {
+        std::vector<LineChunk>& c;
+        ~EventGuard() {
+            for (auto& x : c) {
+                if (x.split) cudaEventDestroy(x.split);
+                if (x.done) cudaEventDestroy(x.done);
+                x.tr.destroy();
+            }
+        }
+    } guard{chunks};
+
+    // as tokenize_lines_impl: chunks c+2, c+3 are copied in and split while chunk c+1 is parsed, scored and evaluated
+    uint64_t lines_issued = 0, lines = 0, tot[kEvalTotals] = {};
+    bool overflow = false;
+    auto stage1 = [&](size_t c) {
+        Scratch& s = *lease[c % kDepth]->s;
+        // per-line counts go out only while the buffer has room for the chunk (its line count is known in the stage)
+        cuda_check(cudaEventSynchronize(chunks[c].split), "sync(split)");
+        const uint64_t n = s.h_totals[2];
+        const bool fits = line_counts && lines_issued + n <= line_capacity;
+        if (line_counts && !fits) overflow = true;
+        eval_stage1(*p, s, chunks[c], no_norm == 0, wsconst_types, tags, tag_mode, fits ? line_counts : nullptr, lines_issued);
+        lines_issued += n;
+    };
+    for (size_t c = 0; c < std::min<size_t>(3, nchunks); ++c) lines_stage0(*lease[c % kDepth]->s, chunks[c], utf8);
+    stage1(0);
+    for (size_t c = 0; c < nchunks; ++c) {
+        if (c + 3 < nchunks) lines_stage0(*lease[(c + 3) % kDepth]->s, chunks[c + 3], utf8);
+        if (c + 1 < nchunks) stage1(c + 1);
+        Scratch& s = *lease[c % kDepth]->s;
+        cuda_check(cudaEventSynchronize(chunks[c].done), "sync(evaluate)");
+        const uint64_t key = s.h_eval[kEvalTotals];
+        if (key != kGoldNoError) {
+            // chunks are checked in line order: the first chunk with an error holds the lowest bad line
+            const uint64_t line = lines + (key >> 34);
+            const uint32_t kind = uint32_t(key & 7u);
+            if (kind == kGoldUtf8)
+                throw Error(kIoError, "stream did not contain valid UTF-8 (line " + std::to_string(line) + ")");
+            throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind) +
+                                              " (line " + std::to_string(line) + ")");
+        }
+        for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
+        lines += chunks[c].n_lines;
+    }
+    for (int i = 0; i < kDepth; ++i)
+        if (lease[i]) {
+            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(evaluate)");
+            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
+        }
+    if (pipeline_trace())
+        for (size_t c = 0; c < nchunks; ++c) chunks[c].tr.print("evaluate", c, chunks[c].nbytes, chunks[0].tr);
+    out->n_lines = lines;
+    out->tp = tot[0];
+    out->tn = tot[1];
+    out->fp = tot[2];
+    out->fn = tot[3];
+    out->n_sys = tot[4];
+    out->n_ref = tot[5];
+    out->n_cor = tot[6];
+    out->n_sentences = tot[7];
+    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: line_capacity: too small for the lines");
+    return kOk;
+    VPT_API_END
 }
 
 namespace {

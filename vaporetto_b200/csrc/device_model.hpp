@@ -140,4 +140,64 @@ cudaError_t launch_tokenize(const TokArgs& t, cudaStream_t stream);
 cudaError_t launch_wsconst(const TokArgs& t, uint8_t* boundaries, uint32_t mask, bool norm, cudaStream_t stream);
 cudaError_t launch_grapheme(const TokArgs& t, uint8_t* boundaries, bool norm, cudaStream_t stream);
 
+// ---- evaluate.cu: gold corpus parsing (Sentence::from_tokenized) and the evaluate metrics ---------------------------
+// error kinds of a gold line, in the low 3 bits of its error key (position in the line + 1) << 3 | kind; a chunk's
+// key is line << 34 | line key, so the smallest key is the first error of the lowest bad line
+constexpr uint64_t kGoldNoError = ~0ull;
+enum GoldError : uint32_t {
+    kGoldUtf8 = 1,       // not valid UTF-8 (BufRead::lines fails before the line is parsed)
+    kGoldEmpty = 2,      // "must contain at least one character" (a lone '\')
+    kGoldStartWs = 3,    // "must not start with a whitespace"
+    kGoldDoubleWs = 4,   // "must not contain consecutive whitespaces"
+    kGoldSlash = 5,      // "a slash must follow a character"
+    kGoldNul = 6,        // "must not contain NULL"
+    kGoldEndWs = 7,      // "must not end with a whitespace"
+};
+// how the system's tags compare with the gold tags (evaluate/src/main.rs:110-120 with predictor.rs:553)
+enum EvalTagMode : int32_t {
+    kTagsAlwaysEqual = 0,  // --no-norm without tag prediction: the sentence keeps the gold tags
+    kTagsGoldEmpty = 1,    // normalised, no tag prediction: empty system tags, equal where the line has no tag field
+    kTagsCompare = 2,      // tag prediction with n_tags > 0: equal where the gold width is n_tags and every slot matches
+};
+constexpr int kEvalTotals = 8;  // tp tn fp fn n_sys n_ref n_cor n_sentences
+
+struct EvalArgs {
+    // the chunk's lines (SplitArgs outputs)
+    const uint8_t* text = nullptr;          // readable up to a multiple of 4 past the end
+    const uint64_t* offsets = nullptr;      // [n_sent + 1]
+    const uint8_t* trims = nullptr;         // [n_sent]
+    uint64_t n_sent = 0;
+    // k_gold_parse outputs
+    uint8_t* surface = nullptr;             // raw sentence text of every line, concatenated
+    uint64_t* surf_offsets = nullptr;       // [n_sent + 1] into surface
+    uint64_t* char_offsets = nullptr;       // [n_sent + 1] first character of every line
+    uint8_t* gold_bnd = nullptr;            // [characters] 1: a word boundary is before the character
+    uint32_t* tag_pos = nullptr;            // nullable [characters]: at a token's last character, the position in text of
+                                            // its first tag '/'; else ~0
+    uint32_t* width = nullptr;              // [n_sent] gold tag width (the sentence's n_tags)
+    uint64_t* state = nullptr;              // [n_groups] look-back scratch
+    uint32_t* ticket = nullptr;             // the 8 bytes after state
+    uint64_t* err = nullptr;                // device scalar: smallest error key (set to kGoldNoError before the launch)
+    // k_eval inputs: the system's sentences (scored on `surface`) and tag records
+    const int32_t* status = nullptr;
+    const uint32_t* n_chars = nullptr;
+    const uint8_t* boundaries = nullptr;    // after the post-filters
+    const uint64_t* bound_offsets = nullptr;
+    int32_t tag_mode = kTagsAlwaysEqual;
+    uint32_t n_tags = 0;                    // kTagsCompare: the model's n_tags; records and strings as in TokArgs
+    const uint64_t* tok_base = nullptr;
+    const int32_t* tok_ids = nullptr;
+    const uint8_t* tok_cands = nullptr;
+    const uint32_t* ts_slot = nullptr;
+    const uint32_t* ts_cand = nullptr;
+    const uint2* ts_ref = nullptr;
+    const uint8_t* ts_bytes = nullptr;
+    // k_eval outputs
+    uint32_t* line_counts = nullptr;        // nullable [n_sent * 7]: tp tn fp fn n_sys n_ref n_cor of every line
+    uint64_t* totals = nullptr;             // [kEvalTotals], added to
+};
+// zeroes state[0 .. n_groups] (ticket included), then parses the lines
+cudaError_t launch_gold_parse(const EvalArgs& e, cudaStream_t stream);
+cudaError_t launch_eval(const EvalArgs& e, cudaStream_t stream);
+
 }  // namespace vpt
