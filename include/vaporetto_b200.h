@@ -220,9 +220,9 @@ int vpt_predict(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_by
  * d_tag_cand[i * n_tags + k] = index of the chosen candidate of tag slot k (else -1): the arrays vpt_fill_tags writes for
  * one sentence.  Token lookup (exact, by bytes), the weight vectors keyed by (pattern id, token, rel position) with the
  * reference's suffix merge (PositionalWeightWithTag +=, predictor.rs:242-262) and the per-slot arg-max (first strict
- * maximum, predictor.rs:286-304) run in one kernel, k_tags.  *d_unserved (nullable, zero it first) counts tokens whose
- * tag model exceeds the limits of the device tables (more than 64 scores or 8 tag slots; none of the reference's
- * models): their entries are -1 and vpt_fill_tags serves them.  Returns VPT_UNSUPPORTED when the whole model is beyond
+ * maximum, predictor.rs:286-304) run in one kernel, k_tags; tokens of any length are served.  *d_unserved (nullable,
+ * zero it first) counts tokens whose own tag model exceeds the limits of the device tables (more than 64 scores or 8 tag
+ * slots; none of the reference's models): their entries are -1 and vpt_fill_tags serves them.  Returns VPT_UNSUPPORTED when the whole model is beyond
  * the limits, VPT_INVALID_ARGUMENT for a predictor created with predict_tags = false (the reference panics). */
 int vpt_predict_tags_batch_dev(const vpt_predictor* predictor, const uint8_t* d_utf8, const uint64_t* d_byte_offsets,
                                size_t n_sent, const int32_t* d_status, const uint8_t* d_boundaries,
@@ -271,8 +271,9 @@ uint32_t vpt_tag_n_tokens(const vpt_predictor* predictor);
  *                      sentences): the token id for vpt_tag_string (-1: the token has no tag model) and, per tag slot,
  *                      the chosen candidate as one byte (255: none) -- `Predictor::predict_tags`, predictor.rs:546-637,
  *                      the same choice vpt_predict_batch_tags reports per character.
- * The totals come back in *n_boundaries_out / *n_tokens_total_out; *n_unserved_out counts tokens whose tag model
- * exceeds the device limits (0 for the reference's models; vpt_fill_tags serves those).  Too small capacities return
+ * The totals come back in *n_boundaries_out / *n_tokens_total_out; *n_unserved_out counts tokens whose own tag model
+ * exceeds the device limits (0 for the reference's models; vpt_fill_tags serves those; the length of a token never
+ * matters).  Too small capacities return
  * InvalidArgument with the totals set. */
 int vpt_predict_batch_compact(const vpt_predictor* predictor, const uint8_t* utf8, const uint64_t* byte_offsets,
                               size_t n_sent, uint32_t* boundary_bits_out, size_t bits_capacity_words,
@@ -347,7 +348,9 @@ int vpt_tokenize_lines(const vpt_predictor* predictor, const uint8_t* utf8, size
  * (sentence.rs:850-886: every token is followed by '/' + tag for its tag slots up to the last one that has a tag, the
  * tag strings escaped like the surface).  Tag prediction (token lookup by the bytes of the pre-filtered token, tag
  * weights, arg-max) and the output with its tag strings run on the device; the predictor must have been created with
- * predict_tags = 1.  `out` needs room for the tags: at most 3 * n_bytes + n_lines + n_bytes * (longest tag suffix). */
+ * predict_tags = 1.  `out` needs room for the tags: at most 3 * n_bytes + n_lines + n_bytes * (longest tag suffix).
+ * Returns VPT_UNSUPPORTED, before writing anything, when the tag model of any token exceeds the limits of the device
+ * tables (see vpt_predict_tags_batch_dev): this path has no per-token fall-back to vpt_fill_tags. */
 int vpt_tokenize_lines_tags(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes, int no_norm,
                             uint32_t wsconst_types, uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
 

@@ -121,6 +121,7 @@ struct vpt_predictor : HostPredictor {
     // device-side tag prediction (tags.hpp): one allocation holding all tables; dt.tok_tab == nullptr when unavailable
     void* d_tags = nullptr;
     DevTags dt;
+    bool tags_all_usable = false;  // every token's own model is within the device limits (TagTablesHost::all_tokens_usable)
     // scratch pool
     mutable std::mutex mu;
     mutable std::vector<std::unique_ptr<Scratch>> pool;
@@ -282,6 +283,7 @@ void upload_tags(vpt_predictor& p) {
     d.max_token_bytes = t.max_token_bytes;
     d.n_char_patterns = uint32_t(p.char_suffix_link.size());
     d.n_type_patterns = uint32_t(p.type_suffix_link.size());
+    p.tags_all_usable = t.all_tokens_usable;
 }
 
 struct ScratchLease {
@@ -1137,7 +1139,8 @@ bool check_lines_flags(const vpt_predictor* p, uint32_t wsconst_types, bool tags
     if (tags) {
         if (!p->predict_tags || p->from_blob)
             throw Error(kInvalidArgument, "InvalidArgumentError: this predictor is created with predict_tags = false");
-        if (p->n_tags && !p->dt.tok_tab)
+        // (these paths have no per-token fall-back: a token the device cannot serve would be written without its tags)
+        if (p->n_tags && (!p->dt.tok_tab || !p->tags_all_usable))
             throw Error(kUnsupported, "this tag model exceeds the limits of the device path (tags.hpp); use vpt_fill_tags");
         if (p->n_tags == 0) tags = false;  // predictor.rs:553-555: nothing to predict
     }

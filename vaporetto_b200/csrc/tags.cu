@@ -2,7 +2,9 @@
 //
 // One warp per sentence walks its characters 32 at a time (the same window decoder as the sentence-warp scorer: it
 // yields the byte position of every character).  A lane whose character ends a token (final boundary after it, or the
-// last character) finds the token's first character by walking back over the boundaries, hashes the token's bytes and
+// last character) takes the byte position of the token's first character from the ring when the token began in the same
+// 32-character step, and otherwise from a warp-uniform carry that the step closing the previous token read from the ring
+// (tokens of any length are located: the ring itself reaches back only ~100 characters), hashes the token's bytes and
 // looks it up in the token table; for a known token it starts from the tag model's bias, adds the weight vectors keyed
 // by (pattern id at characters last .. last + rel, token, rel) of both scorers -- the pattern's own vector plus those of
 // its suffix patterns with the reference's truncation (tags.hpp) -- and takes the first strict maximum of every tag slot
@@ -46,7 +48,7 @@ __global__ void __launch_bounds__(kTagWarps * 32, kLocateOnly ? 8 : 1) k_tags(De
     uint64_t wpos = b0 & ~3ull;
     uint32_t nd = 0;
     uint32_t tok_rank = 0;  // tokens that end before this chunk of characters
-    uint32_t chunk_start = 0;  // first character of the token that is open at the start of the chunk
+    uint32_t open_sb = 0;   // byte position (from b0) of the first character of the token open at the start of the chunk
     for (uint32_t c0 = 0; c0 < n; c0 += 32) {
         // byte positions of the characters up to c0 + 32 (one more: the end of the chunk's last character)
         const uint32_t need = min(n, c0 + 33u);
@@ -65,29 +67,32 @@ __global__ void __launch_bounds__(kTagWarps * 32, kLocateOnly ? 8 : 1) k_tags(De
         uint32_t desc_x = 0, desc_y = 0, desc_z = 0, desc_w = 0;
         if (i < n) {
             if (ends) {
-                // the token starts behind the previous token end: in this chunk (ballot) or before it (carried)
+                // the token starts behind the previous token end: in this chunk (ballot; the ring holds it) or before it (carried)
                 const unsigned before = endm_all & ((1u << lane) - 1u);
-                const uint32_t start = before ? c0 + 32u - uint32_t(__clz(before)) : chunk_start;
-                const bool near = i - start < uint32_t(kRing - 40);  // the ring still holds the token's first character
-                const uint32_t sb = near ? r.bp[start & kRingMask] : 0u;
+                const uint32_t sb = before ? r.bp[(c0 + 32u - uint32_t(__clz(before))) & kRingMask] : open_sb;
                 const uint32_t eb = i + 1 < n ? r.bp[(i + 1) & kRingMask] : uint32_t(b1 - b0);
                 if (kLocateOnly) {
                     // phase 1 of the per-token path: where the token is; k_tok_lookup and k_tok_score do the rest, one thread per token
-                    desc_x = near ? uint32_t(b0 + sb - a.text_base) : 0u;
-                    desc_y = uint32_t((b0 + sb - a.text_base) >> 32);
+                    const uint64_t off = b0 + sb - a.text_base;
+                    desc_x = uint32_t(off);
+                    desc_y = uint32_t(off >> 32) | (min(n - i, 0xFFFFu) << 16);
                     desc_z = uint32_t(cb + i);
-                    desc_w = (near ? min(eb - sb, 0xFFFFu) : 0u) | (min(n - i, 0xFFFFu) << 16);
-                    if (!near && a.n_unserved) atomicAdd(a.n_unserved, 1u);
-                } else if (near) {
-                    if (!kLocateOnly) tok = tag_token_at(t, a.text + b0 + sb, eb - sb, a.char_states ? a.char_states + cb : nullptr,
+                    desc_w = eb - sb;
+                } else {
+                    tok = tag_token_at(t, a.text + b0 + sb, eb - sb, a.char_states ? a.char_states + cb : nullptr,
                                        a.type_states ? a.type_states + cb : nullptr, i, n, cand, a.n_unserved, a.norm);
-                } else if (a.n_unserved) {
-                    atomicAdd(a.n_unserved, 1u);  // a token longer than the ring: left to the host path
                 }
             }
         }
         __syncwarp();
-        if (endm_all) chunk_start = c0 + 32u - uint32_t(__clz(endm_all));
+        if (endm_all) {
+            // The token after this chunk's last token end starts at character `next` <= c0 + 32.  Its ring slot is live
+            // now and is overwritten by a later chunk's decoding: decoding stops once nd >= min(n, c0 + 33) and appends
+            // at most 128 characters per window, so next < nd <= c0 + 160 and the ring holds [nd - 256, nd) with
+            // nd - 256 <= c0 - 96 < next.  (next == n: no token follows.)
+            const uint32_t next = c0 + 32u - uint32_t(__clz(endm_all));
+            if (next < n) open_sb = r.bp[next & kRingMask];
+        }
         if (a.tok_base) {
             // per-token records: the token's rank is the number of boundaries before its last character
             const unsigned endm = endm_all;
@@ -130,10 +135,9 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_lookup(DevTags t, TagArg
         bool listed = false;
         if (rec < ntok) {
             const uint4 d = a.tok_desc[rec];
-            const uint32_t len = d.w & 0xFFFFu;
             int32_t tok = -1;
             uint32_t tid = 0;
-            if (len && token_lookup(t, a.text + a.text_base + ((uint64_t(d.y) << 32) | d.x), len, a.norm, tid)) {
+            if (token_lookup(t, a.text + a.text_base + ((uint64_t(d.y & 0xFFFFu) << 32) | d.x), d.w, a.norm, tid)) {
                 if (__ldg(&t.tok_info[tid].usable)) {
                     tok = int32_t(tid);
                     listed = true;
@@ -166,7 +170,7 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_score(DevTags t, TagArgs
         for (int k = 0; k < kTagMaxSlots; ++k) cand[k] = -1;
         // (characters [d.z, d.z + n_after) are the token's last character and what follows it in its sentence)
         const int32_t tok = tag_score_token(t, uint32_t(a.tok_ids[rec]), a.char_states ? a.char_states + d.z : nullptr,
-                                            a.type_states ? a.type_states + d.z : nullptr, 0, d.w >> 16, cand, a.n_unserved);
+                                            a.type_states ? a.type_states + d.z : nullptr, 0, d.y >> 16, cand, a.n_unserved);
         if (tok < 0) a.tok_ids[rec] = -1;
         for (uint32_t k = 0; k < nt; ++k) a.tok_cands[uint64_t(rec) * nt + k] = (tok >= 0 && cand[k] >= 0) ? uint8_t(cand[k]) : uint8_t(255);
     }

@@ -64,6 +64,7 @@ struct TagChain {        // 16 bytes: patterns 1..4 steps down the suffix chain 
 
 struct TagTablesHost {
     bool usable = false;           // false: some limit is exceeded -> only the host path (vpt_fill_tags) serves the model
+    bool all_tokens_usable = false;  // every TagTokenInfo::usable is set: the device serves every token of the model
     uint32_t n_tags = 0, n_tokens = 0;
     uint32_t tok_mask = 0;         // token table capacity - 1 (power of two)
     uint32_t char_rels = 0, type_rels = 0;   // rel positions 0 .. rels-1 carry weights (window + 1)
@@ -119,16 +120,18 @@ struct TagArgs {
     const uint32_t* type_states = nullptr;
     int32_t* tag_token = nullptr;           // [n_chars] out: token id of the token ending at the character, or -1
     int32_t* tag_cand = nullptr;            // [n_chars * n_tags] out: chosen candidate per slot, or -1
-    uint32_t* n_unserved = nullptr;         // nullable device counter: tokens whose model exceeds the device limits
+    uint32_t* n_unserved = nullptr;         // nullable device counter: tokens whose own model exceeds the device limits
+                                            // (TagTokenInfo::usable == 0) or is malformed; tokens of any length are served
     // per-TOKEN output (vpt_predict_batch_compact) instead of the per-character arrays above: token r of sentence s
     // (in text order) is record tok_base[s] + r
     const uint64_t* tok_base = nullptr;     // [n_sent + 1] exclusive prefix of the tokens per sentence; selects this mode
     int32_t* tok_ids = nullptr;             // [n_tokens] token id or -1
     uint8_t* tok_cands = nullptr;           // [n_tokens * n_tags] chosen candidate per slot, 255 = none
-    // with tok_desc the sentence-warp kernel only LOCATES the tokens (16 bytes each: byte offset from text + text_base,
-    // index of the last character, byte length | characters left in the sentence << 16) and two more kernels, one thread per
-    // token, look the tokens up and predict the tags of those that have a model: full lanes and short dependent-load
-    // chains instead of one sentence per warp
+    // with tok_desc the sentence-warp kernel only LOCATES the tokens (16 bytes each: x = low 32 bits of the byte offset
+    // from text + text_base, y = its bits 32..47 | characters left in the sentence (saturated at 0xFFFF) << 16, z = index
+    // of the last character, w = byte length) and two more kernels, one thread per token, look the tokens up and predict
+    // the tags of those that have a model: full lanes and short dependent-load chains instead of one sentence per warp.
+    // (The offsets index a host buffer's bytes, below 2^47 on every 64-bit host.)
     uint4* tok_desc = nullptr;              // [max_tokens] scratch; nullable (then k_tags does everything itself)
     uint64_t max_tokens = 0;                // bound on the number of tokens (e.g. the number of characters)
     uint32_t* tok_work = nullptr;           // [4 + max_tokens] scratch, needed with tok_desc: [0] counts the tokens that have a

@@ -169,6 +169,7 @@ TagTablesHost build_tag_tables(const HostPredictor& hp) {
     if (t.c_link.empty()) { t.c_link.push_back(kNoPattern); t.c_chain.push_back(TagChain{{kNoPattern, kNoPattern, kNoPattern, kNoPattern}}); }
     if (t.t_link.empty()) { t.t_link.push_back(kNoPattern); t.t_chain.push_back(TagChain{{kNoPattern, kNoPattern, kNoPattern, kNoPattern}}); }
     t.usable = t.keys.size() < (1ull << 32) && t.pool.size() < (1ull << 32);
+    t.all_tokens_usable = std::all_of(t.tok_info.begin(), t.tok_info.end(), [](const TagTokenInfo& ti) { return ti.usable != 0; });
     return t;
 }
 
