@@ -332,7 +332,9 @@ int vpt_write_tokenized_text(const vpt_predictor* predictor, const uint8_t* utf8
  * `out` receives the output lines, each terminated by '\n' (at most 3 * n_bytes + n_lines bytes); *out_len
  * the number of bytes produced (also when `out_capacity` was too small, which returns InvalidArgument);
  * *n_lines the number of input lines.  Chunk size of the internal pipeline: env VPT_CHUNK_BYTES (16 MiB, with
- * smaller chunks at both ends); VPT_TRACE=1 prints the pipeline's per-chunk timeline to stderr. */
+ * smaller chunks at both ends); VPT_TRACE=1 prints the pipeline's per-chunk timeline to stderr.
+ * For input that arrives in pieces or does not fit in memory (a pipe, a file read in pieces, an interactive session),
+ * the line stream below (vpt_line_stream_*, VPT_STREAM_TOKENIZE) gives the same output in bounded memory. */
 #define VPT_WSCONST_DIGIT (1u << 1)    /* --wsconst D */
 #define VPT_WSCONST_ROMAN (1u << 2)    /* --wsconst R */
 #define VPT_WSCONST_HIRAGANA (1u << 3) /* --wsconst H */
@@ -350,7 +352,8 @@ int vpt_tokenize_lines(const vpt_predictor* predictor, const uint8_t* utf8, size
  * weights, arg-max) and the output with its tag strings run on the device; the predictor must have been created with
  * predict_tags = 1.  `out` needs room for the tags: at most 3 * n_bytes + n_lines + n_bytes * (longest tag suffix).
  * Returns VPT_UNSUPPORTED, before writing anything, when the tag model of any token exceeds the limits of the device
- * tables (see vpt_predict_tags_batch_dev): this path has no per-token fall-back to vpt_fill_tags. */
+ * tables (see vpt_predict_tags_batch_dev): this path has no per-token fall-back to vpt_fill_tags.
+ * The line stream (vpt_line_stream_*, VPT_STREAM_TOKENIZE with predict_tags) gives the same output in bounded memory. */
 int vpt_tokenize_lines_tags(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes, int no_norm,
                             uint32_t wsconst_types, uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
 
@@ -375,7 +378,8 @@ int vpt_tokenize_lines_tags(const vpt_predictor* predictor, const uint8_t* utf8,
  * sentence.rs:450), and the counts are 64-bit (the reference's i32 counters wrap beyond 2^31).
  * `predict_tags` and `wsconst_types` are checked as in vpt_tokenize_lines_tags.  `line_counts` (nullable) receives
  * tp, tn, fp, fn, n_sys, n_ref, n_cor of every input line (zeros for empty lines), `line_capacity` rows of 7; a
- * buffer with fewer rows than lines returns VPT_INVALID_ARGUMENT after the totals are filled in. */
+ * buffer with fewer rows than lines returns VPT_INVALID_ARGUMENT after the totals are filled in.
+ * The line stream (vpt_line_stream_*, VPT_STREAM_EVALUATE) gives the same totals on a corpus fed in pieces. */
 typedef struct vpt_eval_counts {
     uint64_t n_lines, n_sentences;       /* input lines; non-empty lines evaluated */
     uint64_t tp, tn, fp, fn;             /* --metric char  (evaluate/src/main.rs:121-147) */
@@ -384,6 +388,57 @@ typedef struct vpt_eval_counts {
 int vpt_evaluate_lines(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes, int no_norm,
                        uint32_t wsconst_types, int predict_tags, vpt_eval_counts* out,
                        uint32_t* line_counts /* nullable, [n_lines * 7] */, uint64_t line_capacity);
+
+/* ---- Line stream: the same loops fed in pieces, for input of any size -------------------------------------------------
+ *
+ * vpt_tokenize_lines, vpt_tokenize_lines_tags and vpt_evaluate_lines take one whole buffer, and their output buffer
+ * grows with it.  A line stream runs the same loops on input fed in pieces of any size, split at any byte, as the
+ * reference's CLIs read stdin line by line: the output is handed back in input order as chunks complete, and host
+ * memory stays bounded by the pipeline depth times the chunk size, plus the longest line.
+ *
+ * Equivalence: for every way of cutting a buffer B into feeds, the stream gives what the whole-buffer call on B with
+ * the same flags gives: the concatenation of the bytes passed to `write`, and *n_lines, equal the output and line
+ * count of vpt_tokenize_lines (vpt_tokenize_lines_tags with predict_tags); the totals, and the error status and message
+ * with its "(line N)", equal those of vpt_evaluate_lines.  Cuts inside a multi-byte character or between '\r' and
+ * '\n', empty feeds, an unterminated last line and a trailing '\r' included: the stream cuts its input only after a
+ * '\n', so every chunk is a run of complete lines.  (A line over 1 GiB is an error in both; the whole-buffer calls
+ * report it before anything else, the stream when it reaches the line.)
+ *
+ * Flags are checked by vpt_line_stream_new with the statuses and messages of the whole-buffer calls (wsconst bits, tags
+ * on a predictor without tags, a tag model beyond the device limits).
+ *
+ * Progress:
+ *  - feed copies the bytes into pinned staging and returns; the caller may reuse its buffer at once.  A chunk is
+ *    submitted once the open chunk reaches the chunk size (env VPT_CHUNK_BYTES, 16 MiB; the first chunks ramp up from
+ *    1/8 of it) and holds a '\n'.  With four chunks in flight, feed waits for the oldest and delivers its output: this
+ *    back-pressure bounds the memory.
+ *  - flush submits every complete line held, waits for all chunks in flight and delivers their output; a partial
+ *    last line stays held.
+ *  - finish submits the rest, an unterminated last line included, and delivers everything.  *n_lines (nullable)
+ *    receives the number of input lines; `counts` (nullable; VPT_STREAM_EVALUATE) the totals of vpt_evaluate_lines.
+ *    There are no per-line counts on the stream.
+ * Memory: one pinned input buffer per chunk in flight plus the open one, a pinned output buffer sized by the largest
+ * chunk output met (tokenize), and the device scratch of four whole-buffer chunks; none of it grows with the total
+ * input, only a line longer than a chunk grows the open buffer.
+ * `write` (VPT_STREAM_TOKENIZE) is called in input order on the thread that called feed / flush / finish, never with
+ * zero bytes; the bytes are valid only during the call.  A nonzero return aborts the stream with VPT_IO_ERROR ("write
+ * callback failed").
+ * Errors poison the stream: after any error (a bad gold line, invalid UTF-8 in evaluate, a line over 1 GiB, a CUDA
+ * error, a failed `write`) every later call returns the same status and message, and `write` is not called again.
+ * feed, flush or finish after finish return VPT_INVALID_ARGUMENT.
+ * vpt_line_stream_free works at any point, finished or not: it waits for the stream's work on the device, calls
+ * nothing back, and leaves the predictor usable.  A stream is used by one thread at a time; several streams on one
+ * predictor (and whole-buffer calls) may run concurrently.  VPT_TRACE=1 prints the stream's per-chunk timeline. */
+typedef struct vpt_line_stream vpt_line_stream;
+typedef int (*vpt_stream_write_fn)(void* ctx, const uint8_t* bytes, size_t n);
+#define VPT_STREAM_TOKENIZE 0 /* vpt_tokenize_lines / _tags output, through `write` */
+#define VPT_STREAM_EVALUATE 1 /* vpt_evaluate_lines totals at finish; `write` unused (may be NULL) */
+int vpt_line_stream_new(const vpt_predictor* predictor, int kind, int no_norm, uint32_t wsconst_types, int predict_tags,
+                        vpt_stream_write_fn write, void* ctx, vpt_line_stream** out);
+int vpt_line_stream_feed(vpt_line_stream* stream, const uint8_t* bytes, size_t n);
+int vpt_line_stream_flush(vpt_line_stream* stream);
+int vpt_line_stream_finish(vpt_line_stream* stream, uint64_t* n_lines, vpt_eval_counts* counts /* EVALUATE only */);
+void vpt_line_stream_free(vpt_line_stream* stream);
 
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */

@@ -10,10 +10,13 @@
 //                                           iter_tokens, write_tokenized_text)
 //   vaporetto::CharacterBoundary / CharacterType   sentence.rs:9-29,70-82
 //   vaporetto::VaporettoError   errors.rs:15-38 (thrown as a C++ exception; `Result<_, VaporettoError>`)
+//   vaporetto::LineStream   (this library's own) tokenize_lines / evaluate_lines on input fed in pieces, output to a sink
 // Where the reference panics (fill_tags on a predictor created with predict_tags = false, predictor.rs:547-551)
 // this mirror throws VaporettoError(InvalidArgument).
 #pragma once
 #include <cstdint>
+#include <exception>
+#include <functional>
 #include <optional>
 #include <stdexcept>
 #include <string>
@@ -335,6 +338,56 @@ private:
     std::vector<std::optional<std::string>> tags_;
     size_t n_tags_ = 0;
     bool tags_filled_ = false;
+};
+
+/// A line stream (`vpt_line_stream_*`): Predictor::tokenize_lines or evaluate_lines on input fed in pieces of any size,
+/// split at any byte, with host memory bounded by the pipeline rather than by the input.  The output goes to `sink` in
+/// input order as chunks complete, on the thread that calls feed / flush / finish; an exception thrown by the sink
+/// aborts the stream and is rethrown from that call.  After any error every call throws it again.
+class LineStream {
+public:
+    using Sink = std::function<void(const uint8_t* bytes, size_t n)>;
+    /// kind: VPT_STREAM_TOKENIZE (`sink` receives the tokenised lines) or VPT_STREAM_EVALUATE (`sink` may be empty).
+    LineStream(const Predictor& predictor, int kind, Sink sink, bool no_norm = false, uint32_t wsconst_types = 0,
+               bool predict_tags = false)
+        : sink_(std::move(sink)) {
+        detail::check(vpt_line_stream_new(predictor.handle(), kind, no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0,
+                                          sink_ ? &LineStream::write : nullptr, this, &h_));
+    }
+    LineStream(const LineStream&) = delete;
+    LineStream& operator=(const LineStream&) = delete;
+    ~LineStream() { vpt_line_stream_free(h_); }
+
+    /// copies the bytes into the stream; delivers the output of the oldest chunk when four are in flight
+    void feed(const void* bytes, size_t n) { check(vpt_line_stream_feed(h_, static_cast<const uint8_t*>(bytes), n)); }
+    void feed(const std::string& bytes) { feed(bytes.data(), bytes.size()); }
+    /// delivers the output of every complete line fed so far
+    void flush() { check(vpt_line_stream_flush(h_)); }
+    /// delivers the rest; returns the number of input lines, `counts` (evaluate) receives the totals
+    uint64_t finish(vpt_eval_counts* counts = nullptr) {
+        uint64_t n = 0;
+        check(vpt_line_stream_finish(h_, &n, counts));
+        return n;
+    }
+
+private:
+    static int write(void* ctx, const uint8_t* bytes, size_t n) {
+        LineStream* self = static_cast<LineStream*>(ctx);
+        try {
+            self->sink_(bytes, n);
+            return 0;
+        } catch (...) {
+            self->error_ = std::current_exception();
+            return 1;
+        }
+    }
+    void check(int rc) {
+        if (error_) std::rethrow_exception(std::exchange(error_, nullptr));
+        detail::check(rc);
+    }
+    Sink sink_;
+    std::exception_ptr error_;
+    vpt_line_stream* h_ = nullptr;
 };
 
 inline void Predictor::predict(Sentence& s) const {

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""The reference's `evaluate` command (evaluate/src/main.rs) on top of vpt_evaluate_lines: a gold corpus in the tokenized
+"""The reference's `evaluate` command (evaluate/src/main.rs) on top of the evaluate line stream (vpt_line_stream_*, the
+loop of vpt_evaluate_lines fed in pieces): a gold corpus in the tokenized
 format on stdin, precision / recall / F1 on stdout, everything between the two (line splitting, gold parsing, full-width
 pre-filter, scoring, --wsconst post-filters, tag prediction, both metrics) on the GPU.
 
@@ -14,6 +15,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+READ_BYTES = 16 << 20  # largest piece read from stdin at once: a corpus of any size is evaluated in bounded memory
 
 
 def rust_f64(x: float) -> str:
@@ -70,10 +72,15 @@ def main(argv=None) -> int:
         model = vb.Model.read_zstd(f.read())
     predictor = vb.Predictor(model, predict_tags=args.predict_tags, device=args.device)
     print("Start tokenization", file=sys.stderr)
-    data = sys.stdin.buffer.read()
     try:
-        counts = predictor.evaluate_lines(data, no_norm=args.no_norm, wsconst="".join(args.wsconst),
-                                          predict_tags=args.predict_tags)
+        with predictor.line_stream("evaluate", no_norm=args.no_norm, wsconst="".join(args.wsconst),
+                                   predict_tags=args.predict_tags) as stream:
+            while True:
+                data = sys.stdin.buffer.read1(READ_BYTES)
+                if not data:
+                    break
+                stream.feed(data)
+            counts = stream.finish()
     except vb.VaporettoError as e:
         print(f"Error: {e}", file=sys.stderr)
         return 1

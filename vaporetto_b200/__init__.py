@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 __all__ = ["Model", "Predictor", "Sentence", "VaporettoError", "CharacterBoundary", "CharacterType", "lib", "build",
-           "BatchResult", "build_blob", "shard_by_bytes"]
+           "BatchResult", "build_blob", "shard_by_bytes", "LineStream"]
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("VPT_B200_LIBRARY") or os.path.join(_PKG, "libvaporetto_b200.so")  # (override: A/B builds)
@@ -120,7 +120,16 @@ ABI = [
     ("vpt_tokenize_lines_tags", C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, C.c_size_t,
                                           C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("vpt_evaluate_lines", C.c_int, [_P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, _P, _P, C.c_uint64]),
+    ("vpt_line_stream_new", C.c_int, [_P, C.c_int, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
+    ("vpt_line_stream_feed", C.c_int, [_P, _P, C.c_size_t]),
+    ("vpt_line_stream_flush", C.c_int, [_P]),
+    ("vpt_line_stream_finish", C.c_int, [_P, C.POINTER(C.c_uint64), _P]),
+    ("vpt_line_stream_free", None, [_P]),
 ]
+
+# vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
+STREAM_WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
+STREAM_KINDS = {"tokenize": 0, "evaluate": 1}
 
 _lib = None
 
@@ -490,6 +499,85 @@ class Predictor:
                                         C.byref(counts), _ptr(lc), 0 if lc is None else lc.shape[0]))
         out = {name: int(getattr(counts, name)) for name, _ in _EvalCounts._fields_}
         return (out, lc) if per_line else out
+
+    def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
+                    predict_tags: bool = False) -> "LineStream":
+        """tokenize_lines (kind="tokenize") or evaluate_lines (kind="evaluate") on input fed in pieces of any size,
+        with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream."""
+        return LineStream(self, kind, no_norm, wsconst, predict_tags)
+
+
+class LineStream:
+    """A line stream (vpt_line_stream_new): the loop of tokenize_lines or evaluate_lines over input fed in pieces, split
+    at any byte.  feed(data) and flush() return the output delivered during the call (bytes; b"" for evaluate);
+    finish() returns (the rest of the output, number of lines) for tokenize and the dict of evaluate_lines for
+    evaluate.  The concatenated output equals the whole-buffer call's on the concatenated input.  flush() delivers the
+    output of every complete line fed so far.  After an error every call raises it again.  Use as a context manager, or
+    call close()."""
+
+    def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool):
+        if kind not in STREAM_KINDS:
+            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize' or 'evaluate'")
+        mask = _wsconst_mask(wsconst)
+        self._predictor = predictor  # (the stream uses the predictor until it is closed)
+        self._kind = kind
+        self._parts: List[bytes] = []
+        self._exc: Optional[BaseException] = None
+        self._write = STREAM_WRITE_FN(self._sink)  # (kept alive as long as the stream)
+        h = _P()
+        _check(lib().vpt_line_stream_new(predictor._h, STREAM_KINDS[kind], int(no_norm), mask, int(predict_tags),
+                                         C.cast(self._write, _P), None, C.byref(h)))
+        self._h = h
+
+    def _sink(self, ctx, data, n):
+        try:
+            self._parts.append(C.string_at(data, n))
+            return 0
+        except BaseException as e:  # re-raised by the call that delivered the output
+            self._exc = e
+            return 1
+
+    def _run(self, fn, *args) -> bytes:
+        if self._h is None:
+            raise VaporettoError(2, "InvalidArgumentError: stream: closed")
+        try:
+            rc = fn(self._h, *args)
+            if self._exc is not None:
+                raise self._exc
+            _check(rc)
+            return b"".join(self._parts)
+        finally:
+            self._parts.clear()
+            self._exc = None
+
+    def feed(self, data) -> bytes:
+        t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
+        return self._run(lib().vpt_line_stream_feed, t.ctypes.data, t.size)
+
+    def flush(self) -> bytes:
+        return self._run(lib().vpt_line_stream_flush)
+
+    def finish(self):
+        n = C.c_uint64()
+        counts = _EvalCounts()
+        out = self._run(lib().vpt_line_stream_finish, C.byref(n), C.byref(counts))
+        if self._kind == "evaluate":
+            return {name: int(getattr(counts, name)) for name, _ in _EvalCounts._fields_}
+        return out, int(n.value)
+
+    def close(self) -> None:
+        h, self._h = getattr(self, "_h", None), None
+        if h and _lib is not None:  # (module globals are already gone when the interpreter shuts down)
+            _lib.vpt_line_stream_free(h)
+
+    def __enter__(self) -> "LineStream":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        self.close()
 
 
 class _EvalCounts(C.Structure):

@@ -7,6 +7,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -19,6 +21,7 @@
 #include "common.hpp"
 #include "device_model.hpp"
 #include "kernel_plan.hpp"
+#include "line_feed.hpp"
 #include "model.hpp"
 #include "predictor_build.hpp"
 #include "grapheme.hpp"
@@ -125,11 +128,14 @@ struct vpt_predictor : HostPredictor {
     // scratch pool
     mutable std::mutex mu;
     mutable std::vector<std::unique_ptr<Scratch>> pool;
+    // pinned staging buffers (pointer, bytes) of line streams that were freed, reused by later streams (under `mu`)
+    mutable std::vector<std::pair<uint8_t*, size_t>> pinned_pool;
 
     ~vpt_predictor() {
         if (d_blob) {
             cudaSetDevice(device);
             pool.clear();
+            for (auto& b : pinned_pool) cudaFreeHost(b.first);
             cudaFree(d_blob);
             if (d_tags) cudaFree(d_tags);
         }
@@ -1441,6 +1447,282 @@ int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_byt
     if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: line_capacity: too small for the lines");
     return kOk;
     VPT_API_END
+}
+
+// ---- line stream: the loops of vpt_tokenize_lines* and vpt_evaluate_lines, fed in pieces ----------------------------
+//
+// The stream cuts its input into chunks of complete lines in pinned staging buffers (line_feed.hpp) and drives every
+// chunk through the per-chunk stages of the whole-buffer drivers, in their order: lines_stage0 (copy-in, newline count),
+// lines_stage1 or eval_stage1 (split, scoring, output or metrics), then the copy-out.  Up to kStreamDepth chunks are in
+// flight, each on its own ScratchLease, so the copy-in, kernels and copy-out of neighbouring chunks overlap.  The
+// whole-buffer drivers keep their own loops: they read the caller's buffer in place, without a staging copy.
+// Invariants: a slot's pinned input buffer is not refilled before its chunk retires, which is after the chunk's `done`
+// event (recorded after its H2D, on the same stream) has completed; the pinned output buffer is not reused before the
+// `write` call that consumed it has returned (chunks retire one at a time, on the caller's thread).
+
+namespace {
+constexpr size_t kStreamDepth = 4;
+}  // namespace
+
+struct vpt_line_stream {
+    struct Slot {
+        std::unique_ptr<ScratchLease> lease;
+        LineChunk ch;
+        FeedBuf in;           // the chunk's pinned input
+        bool stage1 = false;  // lines_stage1 / eval_stage1 issued
+        size_t index = 0;     // chunk number (trace)
+    };
+    const vpt_predictor* p;
+    const int kind;
+    const bool normalize, tags;
+    const uint32_t wsconst;
+    const int tag_mode;
+    const vpt_stream_write_fn write;
+    void* const ctx;
+    const bool trace;
+    const size_t big;               // nominal chunk size (VPT_CHUNK_BYTES)
+    Slot slots[kStreamDepth];
+    std::deque<size_t> fifo;        // slots in flight, oldest first
+    size_t n_chunks = 0;
+    std::vector<FeedBuf> spare;     // input buffers of retired chunks
+    // every pinned buffer of the stream (pointer, bytes); the destructor hands them to the predictor's pool
+    std::vector<std::pair<uint8_t*, size_t>> pinned;
+    FeedBuf out;                    // pinned output staging (tokenize), sized by the largest chunk output seen
+    LineFeed<vpt_line_stream> feed;
+    uint64_t lines = 0, tot[kEvalTotals] = {};
+    TraceEvents t0;                 // trace origin: before the first chunk's copy-in
+    int status = kOk;               // an earlier error: every later call returns it again with `message`
+    std::string message;
+    bool finished = false;
+
+    vpt_line_stream(const vpt_predictor* pr, int k, bool norm, uint32_t ws, bool tg, int tm, vpt_stream_write_fn w, void* c)
+        : p(pr), kind(k), normalize(norm), tags(tg), wsconst(ws), tag_mode(tm), write(w), ctx(c), trace(pipeline_trace()),
+          big(chunk_bytes()), feed(*this, big, kMaxLineChunk) {}
+
+    ~vpt_line_stream() {
+        for (Slot& sl : slots) {
+            sl.lease.reset();  // synchronises the lease's streams and hands its scratch back to the predictor
+            if (sl.ch.split) cudaEventDestroy(sl.ch.split);
+            if (sl.ch.done) cudaEventDestroy(sl.ch.done);
+            sl.ch.tr.destroy();
+        }
+        t0.destroy();
+        // pinning memory costs more than a short stream's work: the buffers of chunk size are kept for later streams
+        // (at most kStreamDepth + 2 per concurrent stream), the others are freed
+        std::lock_guard<std::mutex> g(p->mu);
+        for (const auto& b : pinned) {
+            if (b.second <= 2 * big + big / 2 && p->pinned_pool.size() < 4 * (kStreamDepth + 2)) p->pinned_pool.push_back(b);
+            else cudaFreeHost(b.first);
+        }
+    }
+
+    // a pinned buffer of at least n bytes: from the predictor's pool, else a new one
+    uint8_t* alloc(size_t& n) {
+        {
+            std::lock_guard<std::mutex> g(p->mu);
+            auto& pool = p->pinned_pool;
+            for (size_t i = 0; i < pool.size(); ++i)
+                if (pool[i].second >= n && pool[i].second <= 2 * n) {
+                    const auto b = pool[i];
+                    pool.erase(pool.begin() + long(i));
+                    pinned.push_back(b);
+                    n = b.second;
+                    return b.first;
+                }
+        }
+        void* q = nullptr;
+        cuda_check(cudaMallocHost(&q, n), "cudaMallocHost(stream staging)");
+        pinned.emplace_back(static_cast<uint8_t*>(q), n);
+        return static_cast<uint8_t*>(q);
+    }
+    void release(uint8_t* q) {
+        if (!q) return;
+        pinned.erase(std::find_if(pinned.begin(), pinned.end(), [q](const std::pair<uint8_t*, size_t>& b) { return b.first == q; }));
+        cudaFreeHost(q);
+    }
+
+    // -- LineFeed's host: buffers and chunks
+    FeedBuf fresh(size_t min_cap) {
+        if (spare.empty() && fifo.size() == kStreamDepth) retire();
+        FeedBuf b;
+        if (!spare.empty()) { b = spare.back(); spare.pop_back(); }
+        b.size = 0;
+        if (b.cap < min_cap || b.cap > 2 * std::max(min_cap, big) + big / 2) {
+            // every buffer holds a full chunk, so the ramp at the start allocates nothing twice (a buffer that grew for
+            // a line longer than two chunks is not kept)
+            release(b.data);
+            b.cap = std::max(min_cap, big);
+            b.data = alloc(b.cap);
+        }
+        return b;
+    }
+    void grow(FeedBuf& b, size_t min_cap) {
+        size_t cap = std::max(min_cap, 2 * b.cap);
+        uint8_t* q = alloc(cap);
+        if (b.size) memcpy(q, b.data, b.size);
+        release(b.data);
+        b.data = q;
+        b.cap = cap;
+    }
+    [[noreturn]] void too_long() { throw Error(kInvalidArgument, "InvalidArgumentError: utf8: a line is longer than 1 GiB"); }
+    void emit(FeedBuf& b) {
+        if (fifo.size() == kStreamDepth) retire();
+        const size_t i = n_chunks % kStreamDepth;  // chunks retire in order: this slot is free
+        Slot& sl = slots[i];
+        sl.in = b;
+        b = FeedBuf();
+        if (!sl.lease) sl.lease.reset(new ScratchLease(*p));
+        sl.ch.byte_lo = 0;
+        sl.ch.nbytes = sl.in.size;
+        sl.ch.n_lines = 0;
+        sl.stage1 = false;
+        sl.index = n_chunks++;
+        Scratch& s = *sl.lease->s;
+        if (trace && sl.index == 0) t0.mark(0, s.stream);
+        fifo.push_back(i);
+        lines_stage0(s, sl.ch, sl.in.data);
+        // as in the whole-buffer drivers, the two newest chunks are copied in and counted ahead of their kernels
+        for (size_t k = 0; k + 2 < fifo.size(); ++k)
+            if (!slots[fifo[k]].stage1) issue(slots[fifo[k]]);
+    }
+
+    void issue(Slot& sl) {
+        Scratch& s = *sl.lease->s;
+        if (kind == VPT_STREAM_TOKENIZE) lines_stage1(*p, s, sl.ch, normalize, wsconst, tags);
+        else eval_stage1(*p, s, sl.ch, normalize, wsconst, tags, tag_mode, nullptr, 0);
+        sl.stage1 = true;
+    }
+
+    // waits for the oldest chunk and delivers it: its output to `write` (tokenize) or its totals (evaluate)
+    void retire() {
+        // the next chunk's kernels are queued before the host waits for the oldest
+        for (size_t k = 0; k < std::min<size_t>(2, fifo.size()); ++k)
+            if (!slots[fifo[k]].stage1) issue(slots[fifo[k]]);
+        Slot& sl = slots[fifo.front()];
+        Scratch& s = *sl.lease->s;
+        cuda_check(cudaEventSynchronize(sl.ch.done), "sync(stream)");
+        uint64_t nb = 0;
+        if (kind == VPT_STREAM_TOKENIZE) {
+            nb = s.h_totals[3];
+            if (nb > out.cap) {
+                release(out.data);
+                out.cap = std::max(size_t(nb + nb / 4), big + big / 2);
+                out.data = alloc(out.cap);
+            }
+            if (nb) cuda_check(cudaMemcpyAsync(out.data, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
+            if (trace) sl.ch.tr.mark(3, s.stream_out);
+            cuda_check(cudaStreamSynchronize(s.stream_out), "sync(copy-out)");
+        } else {
+            // chunks retire in line order: the first chunk with an error holds the lowest bad line (as vpt_evaluate_lines
+            // reports it)
+            const uint64_t key = s.h_eval[kEvalTotals];
+            if (key != kGoldNoError) {
+                const uint64_t line = lines + (key >> 34);
+                const uint32_t kind_ = uint32_t(key & 7u);
+                if (kind_ == kGoldUtf8)
+                    throw Error(kIoError, "stream did not contain valid UTF-8 (line " + std::to_string(line) + ")");
+                throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind_) +
+                                                  " (line " + std::to_string(line) + ")");
+            }
+            for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
+        }
+        if (trace) sl.ch.tr.print("stream", sl.index, sl.ch.nbytes, t0);
+        lines += sl.ch.n_lines;
+        fifo.pop_front();
+        spare.push_back(sl.in);
+        sl.in = FeedBuf();
+        if (nb && write(ctx, out.data, size_t(nb)) != 0) throw Error(kIoError, "write callback failed");
+    }
+
+    void drain() {
+        while (!fifo.empty()) retire();
+    }
+};
+
+namespace {
+
+// Runs `f` on a live stream: an error poisons the stream, and every later call returns it again.
+int stream_call(vpt_line_stream* st, const std::function<void()>& f) {
+    if (!st) return fail(Error(kInvalidArgument, "InvalidArgumentError: stream: must not be NULL"));
+    if (st->status != kOk) {
+        set_last_error(st->message);
+        return st->status;
+    }
+    if (st->finished) return fail(Error(kInvalidArgument, "InvalidArgumentError: stream: already finished"));
+    try {
+        cuda_check(cudaSetDevice(st->p->device), "cudaSetDevice");
+        f();
+        return kOk;
+    } catch (const Error& e) {
+        st->status = e.code;
+        st->message = e.what();
+    } catch (const std::exception& e) {
+        st->status = kInternal;
+        st->message = std::string("internal error: ") + e.what();
+    }
+    set_last_error(st->message);
+    return st->status;
+}
+
+}  // namespace
+
+int vpt_line_stream_new(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst_types, int predict_tags,
+                        vpt_stream_write_fn write, void* ctx, vpt_line_stream** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    if (kind != VPT_STREAM_TOKENIZE && kind != VPT_STREAM_EVALUATE)
+        throw Error(kInvalidArgument, "InvalidArgumentError: kind: VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE");
+    const bool tags = check_lines_flags(p, wsconst_types, predict_tags != 0);
+    if (kind == VPT_STREAM_TOKENIZE && !write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
+    // as vpt_evaluate_lines: the system keeps the gold tags (no_norm) or has none, unless tags are predicted
+    const int tag_mode = tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty;
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    *out = new vpt_line_stream(p, kind, no_norm == 0, wsconst_types, tags, tag_mode, write, ctx);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_line_stream_feed(vpt_line_stream* st, const uint8_t* bytes, size_t n) {
+    return stream_call(st, [&] {
+        if (n && !bytes) throw Error(kInvalidArgument, "InvalidArgumentError: bytes: must not be NULL");
+        st->feed.feed(bytes, n);
+    });
+}
+
+int vpt_line_stream_flush(vpt_line_stream* st) {
+    return stream_call(st, [&] {
+        st->feed.flush();
+        st->drain();
+    });
+}
+
+int vpt_line_stream_finish(vpt_line_stream* st, uint64_t* n_lines, vpt_eval_counts* counts) {
+    if (n_lines) *n_lines = 0;
+    if (counts) *counts = vpt_eval_counts();
+    return stream_call(st, [&] {
+        st->feed.finish();
+        st->drain();
+        st->finished = true;
+        if (n_lines) *n_lines = st->lines;
+        if (counts && st->kind == VPT_STREAM_EVALUATE) {
+            counts->n_lines = st->lines;
+            counts->tp = st->tot[0];
+            counts->tn = st->tot[1];
+            counts->fp = st->tot[2];
+            counts->fn = st->tot[3];
+            counts->n_sys = st->tot[4];
+            counts->n_ref = st->tot[5];
+            counts->n_cor = st->tot[6];
+            counts->n_sentences = st->tot[7];
+        }
+    });
+}
+
+void vpt_line_stream_free(vpt_line_stream* st) {
+    if (!st) return;
+    cudaSetDevice(st->p->device);
+    delete st;
 }
 
 namespace {
