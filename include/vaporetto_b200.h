@@ -440,6 +440,50 @@ int vpt_line_stream_flush(vpt_line_stream* stream);
 int vpt_line_stream_finish(vpt_line_stream* stream, uint64_t* n_lines, vpt_eval_counts* counts /* EVALUATE only */);
 void vpt_line_stream_free(vpt_line_stream* stream);
 
+/* ---- Token spans: vaporetto_tantivy's token_stream for a batch of documents ---------------------------------------
+ *
+ * `VaporettoTokenizer::token_stream` (vaporetto_tantivy/src/lib.rs:157-229) on the device, for many documents: only text
+ * goes in and only token byte offsets (and optional tag records) come out.
+ *  - Documents.  Document d is utf8[byte_offsets[d] .. byte_offsets[d+1]).  It is one Sentence: '\r' and '\n' are ordinary
+ *    characters in it (type Other), not line ends.
+ *  - Filters.  The chain of token_stream, in this order:
+ *      1. KyteaFullwidthFilter as the pre-filter, unless `no_norm` (the adapter always applies it; `no_norm` is there for
+ *         parity with the CLI);
+ *      2. predict;
+ *      3. SplitLinebreaksFilter (vaporetto_rules/src/sentence_filters/split_linebreaks.rs:9-37), always: the boundary on
+ *         either side of every '\r' / '\n' becomes WordBoundary;
+ *      4. the `wsconst_types` post-filters (VPT_WSCONST_*, the bit set of vpt_tokenize_lines).
+ *    The line-break split is the only filter that sets boundaries and the wsconst filters only clear them, so D/R/H/T/K/O/G
+ *    commute with each other but not with it: "。\n" under O is one token, and so is "\r\n" under G.
+ *  - Output.  Token r of document d is record T_d + r, T_d = the sum of n_tokens_out over the earlier documents.
+ *    token_ends_out[T_d + r] is the byte offset, from the document's first byte, of the token's exclusive end; its start
+ *    is the previous token's end (0 for the first).  The last end is the document's byte length: the tokens tile the
+ *    document.  This is `boundary_pos` (lib.rs:179-188); a token's `position` is r and its `position_length` is
+ *    n_tokens_out[d] (lib.rs:207-219).
+ *  - Empty and rejected documents.  An empty document has 0 tokens and status VPT_SENT_EMPTY (the adapter returns no
+ *    token for ""); a document with U+0000 or invalid UTF-8 has 0 tokens and status VPT_SENT_NUL / VPT_SENT_BAD_UTF8
+ *    (the adapter panics on NUL: a documented difference).  status_out[d] as in vpt_predict_batch_compact.
+ *  - Tags.  With token_ids_out (the predictor needs predict_tags = 1), token_ids_out / token_cands_out receive the
+ *    records of vpt_predict_batch_compact, one per token: the token id (-1: no tag model) and per tag slot the chosen
+ *    candidate as one byte (255: none).  They are predicted after the post-filters, on the pre-filtered token bytes when
+ *    normalising, as vpt_tokenize_lines_tags predicts them; the flags are checked as there, with the same statuses and
+ *    messages (a model with no tag slots gives -1 for every token).  The adapter itself predicts no tags.
+ *  - Capacity and limits.  token_capacity is the number of records the token arrays hold; an upper bound is the total
+ *    number of bytes.  If it is too small the call returns VPT_INVALID_ARGUMENT with *n_tokens_total_out set to the
+ *    number needed.  A document over 1 GiB is VPT_INVALID_ARGUMENT before anything runs; n_docs == 0 is OK.
+ * The documents flow through the pipeline of vpt_predict_batch_compact (four chunks in flight); a chunk closes at env
+ * VPT_CHUNK_SENTENCES documents (262144) or at env VPT_CHUNK_BYTES of text (16 MiB), whichever comes first, both
+ * ramping up over the first chunks, and a larger document is a chunk by itself.  VPT_TRACE=1 prints the per-chunk
+ * timeline under the tag "spans". */
+int vpt_token_spans(const vpt_predictor* predictor, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_docs,
+                    int no_norm, uint32_t wsconst_types,
+                    uint32_t* n_tokens_out,      /* [n_docs] */
+                    uint8_t* status_out,         /* [n_docs], VPT_SENT_* */
+                    uint32_t* token_ends_out,    /* [token_capacity] */
+                    int32_t* token_ids_out,      /* nullable: tag prediction, as vpt_predict_batch_compact */
+                    uint8_t* token_cands_out,    /* nullable: [token_capacity * n_tags] */
+                    size_t token_capacity, uint64_t* n_tokens_total_out);
+
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */
 uint32_t vpt_kytea_fullwidth(uint32_t code_point);

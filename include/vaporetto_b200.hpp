@@ -203,6 +203,46 @@ public:
         return r;
     }
 
+    /// Result of `token_spans`: see `vpt_token_spans` (include/vaporetto_b200.h).
+    struct SpansResult {
+        std::vector<uint32_t> n_tokens;        // per document
+        std::vector<uint8_t> status;           // per document, VPT_SENT_*
+        std::vector<uint64_t> token_base;      // n_documents + 1: first token record of every document
+        std::vector<uint32_t> token_ends;      // per token: exclusive end, in bytes from its document's start
+        std::vector<int32_t> token_ids;        // per token (tags requested)
+        std::vector<uint8_t> token_cands;      // per token x n_tags, 255 = none
+        /// [from, to) byte offsets of token r of document d
+        std::pair<uint32_t, uint32_t> span(size_t d, size_t r) const {
+            const size_t i = size_t(token_base[d]) + r;
+            return {r ? token_ends[i - 1] : 0u, token_ends[i]};
+        }
+    };
+    /// vaporetto_tantivy's `token_stream` (lib.rs:157-229; `vpt_token_spans`) for documents given as concatenated UTF-8 +
+    /// byte offsets: the full-width pre-filter (unless `no_norm`), predict, the line-break split and the `wsconst_types`
+    /// post-filters on the device; the token byte spans (+ tag records when `tags`) come back.
+    SpansResult token_spans(const std::string& text, const std::vector<uint64_t>& byte_offsets, bool no_norm = false,
+                            uint32_t wsconst_types = 0, bool tags = false) const {
+        SpansResult r;
+        const size_t n = byte_offsets.empty() ? 0 : byte_offsets.size() - 1;
+        const size_t cap = text.size() + 1;  // a token has at least one byte
+        r.n_tokens.assign(n, 0);
+        r.status.assign(n, 0);
+        r.token_ends.assign(cap, 0);
+        const size_t nt = tags ? size_t(info_.n_tags) : 0;
+        if (tags) { r.token_ids.assign(cap, -1); r.token_cands.assign(cap * (nt ? nt : 1), 255); }
+        uint64_t ntok = 0;
+        if (n)
+            detail::check(vpt_token_spans(h_, reinterpret_cast<const uint8_t*>(text.data()), byte_offsets.data(), n,
+                                          no_norm ? 1 : 0, wsconst_types, r.n_tokens.data(), r.status.data(),
+                                          r.token_ends.data(), tags ? r.token_ids.data() : nullptr,
+                                          tags ? r.token_cands.data() : nullptr, cap, &ntok));
+        r.token_ends.resize(size_t(ntok));
+        if (tags) { r.token_ids.resize(size_t(ntok)); r.token_cands.resize(size_t(ntok) * nt); }
+        r.token_base.assign(n + 1, 0);
+        for (size_t d = 0; d < n; ++d) r.token_base[d + 1] = r.token_base[d] + r.n_tokens[d];
+        return r;
+    }
+
     const vpt_predictor_info& info() const { return info_; }
     const vpt_predictor* handle() const { return h_; }
 

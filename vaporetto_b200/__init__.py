@@ -13,7 +13,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 __all__ = ["Model", "Predictor", "Sentence", "VaporettoError", "CharacterBoundary", "CharacterType", "lib", "build",
-           "BatchResult", "build_blob", "shard_by_bytes", "LineStream"]
+           "BatchResult", "build_blob", "shard_by_bytes", "LineStream", "SpansResult", "SpanToken", "Tokenizer"]
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("VPT_B200_LIBRARY") or os.path.join(_PKG, "libvaporetto_b200.so")  # (override: A/B builds)
@@ -125,6 +125,8 @@ ABI = [
     ("vpt_line_stream_flush", C.c_int, [_P]),
     ("vpt_line_stream_finish", C.c_int, [_P, C.POINTER(C.c_uint64), _P]),
     ("vpt_line_stream_free", None, [_P]),
+    ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
+                                  C.POINTER(C.c_uint64)]),
 ]
 
 # vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
@@ -500,6 +502,30 @@ class Predictor:
         out = {name: int(getattr(counts, name)) for name, _ in _EvalCounts._fields_}
         return (out, lc) if per_line else out
 
+    def token_spans(self, text, offsets, no_norm: bool = False, wsconst: str = "", tags: bool = False) -> "SpansResult":
+        """vaporetto_tantivy's token_stream (lib.rs:157-229) for a batch of documents on the device (vpt_token_spans):
+        document d is text[offsets[d]:offsets[d + 1]] (bytes or uint8 array, UTF-8); it is pre-filtered (unless
+        `no_norm`), predicted, split on both sides of every '\r' / '\n' and post-filtered by the `wsconst` letters
+        (D, R, H, T, K, O, G).  `tags`: the tag records of every token (needs predict_tags).  See SpansResult."""
+        mask = _wsconst_mask(wsconst)
+        t = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text, np.uint8)
+        off = np.ascontiguousarray(offsets, np.uint64)
+        n = off.size - 1
+        cap = max(int(off[-1] - off[0]) if n > 0 else 0, 1)  # a token has at least one byte
+        nt = self.n_tags if tags else 0
+        n_tokens = np.zeros(max(n, 1), np.uint32)
+        status = np.zeros(max(n, 1), np.uint8)
+        ends = np.empty(cap, np.uint32)
+        tok = np.empty(cap, np.int32) if tags else None
+        cand = np.empty(cap * max(nt, 1), np.uint8) if tags else None
+        total = C.c_uint64()
+        _check(lib().vpt_token_spans(self._h, t.ctypes.data, off.ctypes.data, max(n, 0), int(no_norm), mask,
+                                     n_tokens.ctypes.data, status.ctypes.data, ends.ctypes.data, _ptr(tok), _ptr(cand),
+                                     cap, C.byref(total)))
+        k = int(total.value)
+        return SpansResult(n_tokens[:max(n, 0)], status[:max(n, 0)], ends[:k], None if tok is None else tok[:k],
+                           None if cand is None else cand[: k * max(nt, 1)].reshape(-1, max(nt, 1))[:, :nt])
+
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False) -> "LineStream":
         """tokenize_lines (kind="tokenize") or evaluate_lines (kind="evaluate") on input fed in pieces of any size,
@@ -614,6 +640,81 @@ class CompactResult:
         lo, hi = (0, self.n_boundaries) if s is None else (int(self.bit_offsets[s]), int(self.bit_offsets[s + 1]))
         out = np.empty(hi - lo, np.uint8)
         _check(lib().vpt_unpack_boundaries(self.boundary_bits.ctypes.data, lo, hi - lo, out.ctypes.data))
+        return out
+
+
+class SpansResult:
+    """Result of Predictor.token_spans: `n_tokens` and `status` (VPT_SENT_*: 0 ok, 1 empty, 2 NUL, 3 invalid UTF-8) per
+    document, `token_base` (n_docs + 1, uint64) the first token record of every document, `token_ends` (uint32) the byte
+    offset of every token's exclusive end from its document's start, and with tags `token_ids` (int32, -1: no tag model)
+    and `token_cands` (uint8 [tokens, n_tags], 255: none)."""
+
+    def __init__(self, n_tokens, status, token_ends, token_ids, token_cands):
+        self.n_tokens, self.status, self.token_ends = n_tokens, status, token_ends
+        self.token_ids, self.token_cands = token_ids, token_cands
+        self.token_base = np.concatenate(([0], np.cumsum(n_tokens.astype(np.uint64)))).astype(np.uint64)
+
+    def spans(self, d: int) -> np.ndarray:
+        """[from, to) byte offsets of the tokens of document d, as a (k, 2) uint32 array."""
+        ends = self.token_ends[int(self.token_base[d]): int(self.token_base[d + 1])]
+        out = np.empty((ends.size, 2), np.uint32)
+        out[:, 1] = ends
+        out[:1, 0] = 0
+        out[1:, 0] = ends[:-1]
+        return out
+
+
+class SpanToken:
+    """`tantivy::tokenizer::Token` as vaporetto_tantivy's token stream fills it (lib.rs:207-219): the token's text, its
+    byte offsets [offset_from, offset_to) in the document, its position, and position_length = the document's number of
+    tokens."""
+    __slots__ = ("text", "offset_from", "offset_to", "position", "position_length")
+
+    def __init__(self, text: str, offset_from: int, offset_to: int, position: int, position_length: int):
+        self.text, self.offset_from, self.offset_to = text, offset_from, offset_to
+        self.position, self.position_length = position, position_length
+
+    def _key(self):
+        return (self.text, self.offset_from, self.offset_to, self.position, self.position_length)
+
+    def __eq__(self, other):
+        return isinstance(other, SpanToken) and self._key() == other._key()
+
+    def __repr__(self):
+        return "SpanToken(text=%r, offset_from=%d, offset_to=%d, position=%d, position_length=%d)" % self._key()
+
+
+_SENT_MESSAGES = {1: "InvalidArgumentError: text: must contain at least one character",
+                  2: "InvalidArgumentError: text: must not contain NULL",
+                  3: "InvalidArgumentError: text: must be valid UTF-8"}
+
+
+class Tokenizer:
+    """`vaporetto_tantivy::VaporettoTokenizer` (lib.rs:54-155) over a device predictor: the full-width pre-filter,
+    predict, SplitLinebreaksFilter and the `wsconst` post-filters (letters D, R, H, T, K, O, G; another letter raises
+    "Could not parse a wsconst value", lib.rs:69-85).  token_stream(text) returns the adapter's tokens; token_streams(texts)
+    those of many documents from one device call (Predictor.token_spans)."""
+
+    def __init__(self, predictor: "Predictor", wsconst: str = ""):
+        if any(ch not in "DRHTKOG" for ch in wsconst):
+            raise VaporettoError(2, "Could not parse a wsconst value")
+        self.predictor, self.wsconst = predictor, wsconst
+
+    def token_stream(self, text: str) -> List[SpanToken]:
+        return self.token_streams([text])[0]
+
+    def token_streams(self, texts: Sequence[str]) -> List[List[SpanToken]]:
+        enc = [t.encode("utf-8") for t in texts]
+        off = np.zeros(len(enc) + 1, np.uint64)
+        np.cumsum([len(e) for e in enc], out=off[1:])
+        r = self.predictor.token_spans(b"".join(enc), off, wsconst=self.wsconst)
+        out = []
+        for d, e in enumerate(enc):
+            st = int(r.status[d])
+            if st >= 2:  # (the adapter panics on NUL; a str cannot hold invalid UTF-8)
+                raise VaporettoError(2, f"{_SENT_MESSAGES[st]} (document {d})")
+            sp = r.spans(d).tolist()
+            out.append([SpanToken(e[a:b].decode("utf-8"), a, b, k, len(sp)) for k, (a, b) in enumerate(sp)])
         return out
 
 

@@ -74,6 +74,7 @@ struct Scratch {
     void* d_tokwork = nullptr; size_t tokwork_cap = 0;  // work list of the per-token tag kernels (TagArgs::tok_work)
     void* d_toklocal = nullptr; size_t toklocal_cap = 0;
     void* d_tokblk = nullptr; size_t tokblk_cap = 0;
+    void* d_ends = nullptr; size_t ends_cap = 0;   // token byte ends (vpt_token_spans)
     // gold corpus and metrics (vpt_evaluate_lines)
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
@@ -90,7 +91,7 @@ struct Scratch {
     void* d_io = nullptr;          // its device twin
     ~Scratch() {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
-                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk,
+                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends,
                         d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
@@ -2249,6 +2250,226 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
     if (n_tokens_total_out) *n_tokens_total_out = tok_total;
     if (n_unserved_out) *n_unserved_out = unserved_total;
     if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: bits_capacity_words/token_capacity: too small for the batch");
+    return kOk;
+    VPT_API_END
+}
+
+namespace {
+
+// Pipeline chunks of vpt_token_spans as (first document, documents): the document counts of the ramp schedule over
+// chunk_sentences(), each cut again where its text would pass the byte budget (VPT_CHUNK_BYTES, ramping up from 1/8 of
+// it over the first chunks), whichever comes first.  A document over the budget is a chunk by itself.
+std::vector<std::pair<size_t, size_t>> span_chunks(const uint64_t* byte_offsets, size_t n_docs) {
+    const size_t cs = chunk_sentences();
+    const uint64_t big = chunk_bytes();
+    std::vector<std::pair<size_t, size_t>> out;
+    size_t lo = 0;
+    for (size_t sz : ramp_schedule(n_docs, cs, cs / 8, cs / 4)) {
+        const size_t end = lo + sz;
+        while (lo < end) {
+            const uint64_t budget = out.size() < 3 ? std::max<uint64_t>(big >> (3 - out.size()), 1) : big;
+            // the last document whose end is within the budget (at least one document)
+            size_t hi = size_t(std::upper_bound(byte_offsets + lo + 1, byte_offsets + end + 1, byte_offsets[lo] + budget) -
+                               byte_offsets) - 1;
+            if (hi <= lo) hi = lo + 1;
+            out.emplace_back(lo, hi - lo);
+            lo = hi;
+        }
+    }
+    return out;
+}
+
+}  // namespace
+
+int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_docs, int no_norm,
+                    uint32_t wsconst_types, uint32_t* n_tokens_out, uint8_t* status_out, uint32_t* token_ends_out,
+                    int32_t* token_ids_out, uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_tokens_total_out) {
+    VPT_API_BEGIN
+    if (n_tokens_total_out) *n_tokens_total_out = 0;
+    const bool want_tags = token_ids_out != nullptr || token_cands_out != nullptr;
+    const bool tags = check_lines_flags(p, wsconst_types, want_tags);  // false with n_tags == 0: every token id is -1
+    const size_t nt = tags ? p->n_tags : 0;
+    if (want_tags && (!token_ids_out || (nt && !token_cands_out)))
+        throw Error(kInvalidArgument, "InvalidArgumentError: token_ids_out/token_cands_out: must not be NULL");
+    if (!byte_offsets || !n_tokens_out || !status_out)
+        throw Error(kInvalidArgument, "InvalidArgumentError: byte_offsets/n_tokens_out/status_out: must not be NULL");
+    if (n_docs == 0) return kOk;
+    for (size_t d = 0; d < n_docs; ++d) {
+        if (byte_offsets[d + 1] < byte_offsets[d])
+            throw Error(kInvalidArgument, "InvalidArgumentError: byte_offsets: must be non-decreasing");
+        if (byte_offsets[d + 1] - byte_offsets[d] > kMaxLineChunk)
+            throw Error(kInvalidArgument, "InvalidArgumentError: utf8: a document is longer than 1 GiB");
+    }
+    if (byte_offsets[n_docs] > byte_offsets[0] && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    const bool normalize = no_norm == 0;
+    DevModel dm = p->dm;
+    dm.kytea_norm = normalize ? 1 : 0;
+
+    // Three host-side stages, as in vpt_predict_batch_compact:
+    //   A  copy-in + count pass                  -> boundaries / characters of the chunk (pinned host words)
+    //   B  scoring, line breaks, post-filters, token counts + prefix, (tags), token ends -> tokens of the chunk (pinned)
+    //   C  copy-out (per-document words, token ends and tag records at the running token total)
+    const std::vector<std::pair<size_t, size_t>> cuts = span_chunks(byte_offsets, n_docs);
+    const size_t nchunks = cuts.size();
+    constexpr int kDepth = 4;
+    std::unique_ptr<ScratchLease> lease[kDepth];
+    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
+    struct SChunk {
+        ChunkState cs;
+        cudaEvent_t kernels = nullptr;
+        bool issued = false;
+    };
+    std::vector<SChunk> chunks(nchunks);
+    struct EventGuard {
+        std::vector<SChunk>& c;
+        ~EventGuard() { for (auto& x : c) { if (x.cs.counted) cudaEventDestroy(x.cs.counted); if (x.kernels) cudaEventDestroy(x.kernels); x.cs.tr.destroy(); } }
+    } guard{chunks};
+    for (size_t c = 0; c < nchunks; ++c) {
+        ChunkState& ch = chunks[c].cs;
+        ch.s_lo = cuts[c].first;
+        ch.n = cuts[c].second;
+        ch.byte_lo = byte_offsets[ch.s_lo];
+        ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
+    }
+    uint64_t tok_total = 0;
+    bool overflow = false;
+
+    auto stage_b = [&](size_t c) {
+        SChunk& cc = chunks[c];
+        ChunkState& ch = cc.cs;
+        Scratch& s = *lease[c % kDepth]->s;
+        cudaStream_t st = s.stream;
+        cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
+        const uint64_t nb = s.h_totals[0], nc = s.h_totals[1];
+        if (!cc.kernels) cuda_check(cudaEventCreateWithFlags(&cc.kernels, cudaEventDisableTiming), "cudaEventCreate");
+        BatchArgs& a = ch.a;
+        Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
+        a.scores = nullptr;
+        if (!scores_optional(dm)) {
+            Scratch::ensure(s.d_scores, s.scores_cap, 4 * nb + 4);
+            a.scores = static_cast<int32_t*>(s.d_scores);
+        }
+        a.boundaries = static_cast<uint8_t*>(s.d_bounds);
+        if (tags) {
+            Scratch::ensure(s.d_cst, s.cst_cap, 4 * nc + 4);
+            Scratch::ensure(s.d_tst, s.tst_cap, 4 * nc + 4);
+            a.char_states = static_cast<uint32_t*>(s.d_cst);
+            a.type_states = static_cast<uint32_t*>(s.d_tst);
+        }
+        // (chunk-local offsets: bound_base / char_base stay 0)
+        if (pipeline_trace()) ch.tr.mark(1, st);
+        cuda_check(launch_score(dm, a, st), "launch(score)");
+        if (pipeline_trace()) ch.tr.mark_sub(0, st);  // after the scoring kernel
+        SpanArgs g;
+        g.text = a.text;
+        g.offsets = a.offsets;
+        g.n_sent = ch.n;
+        g.status = a.status;
+        g.n_chars = a.n_chars;
+        g.boundaries = a.boundaries;
+        g.bound_offsets = a.bound_offsets;
+        cuda_check(launch_split_linebreaks(g, st), "launch(split linebreaks)");
+        TokArgs t;
+        t.text = a.text;
+        t.offsets = a.offsets;
+        t.n_sent = ch.n;
+        t.status = a.status;
+        t.n_chars = a.n_chars;
+        t.boundaries = a.boundaries;
+        t.bound_offsets = a.bound_offsets;
+        cuda_check(launch_wsconst(t, a.boundaries, wsconst_types, normalize, st), "launch(wsconst)");
+        if (wsconst_types & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
+        Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
+        Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * ch.n + 16);
+        Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (ch.n + 1) + 16);
+        Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * ch.n + 16);
+        Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (ch.n / kSpanDocs + 4));
+        g.status8 = static_cast<uint8_t*>(s.d_st8);
+        g.n_tokens = static_cast<uint32_t*>(s.d_ntok);
+        g.tok_base = static_cast<uint64_t*>(s.d_tokbase);
+        g.tok_local = static_cast<uint32_t*>(s.d_toklocal);
+        g.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+        g.tok_total_host = &s.h_totals[4];
+        s.h_totals[4] = 0;
+        cuda_check(launch_span_count(g, st), "launch(span count)");
+        if (pipeline_trace()) ch.tr.mark_sub(1, st);  // after the filters and the token counts
+        if (tags) {
+            // tag prediction on the final boundaries, tokens looked up by their pre-filtered bytes (as vpt_tokenize_lines_tags)
+            Scratch::ensure(s.d_tok, s.tok_cap, 4 * nc + 16);
+            Scratch::ensure(s.d_cand, s.cand_cap, nc * std::max<size_t>(nt, 1) + 16);
+            Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * nc + 16);
+            Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nc + 32);
+            TagArgs ta;
+            ta.text = a.text;
+            ta.offsets = a.offsets;
+            ta.n_sent = ch.n;
+            ta.status = a.status;
+            ta.boundaries = a.boundaries;
+            ta.bound_offsets = a.bound_offsets;
+            ta.char_offsets = a.char_offsets;
+            ta.char_states = p->dt.char_rels ? a.char_states : nullptr;
+            ta.type_states = p->dt.type_rels ? a.type_states : nullptr;
+            ta.tok_base = g.tok_base;
+            ta.tok_ids = static_cast<int32_t*>(s.d_tok);
+            ta.tok_cands = static_cast<uint8_t*>(s.d_cand);
+            ta.tok_desc = static_cast<uint4*>(s.d_tokdesc);
+            ta.max_tokens = nc;
+            ta.tok_work = static_cast<uint32_t*>(s.d_tokwork);
+            ta.text_base = 0;
+            ta.norm = normalize ? 1 : 0;
+            cuda_check(launch_tags(p->dt, ta, st), "launch(tags)");
+        }
+        Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
+        g.token_ends = static_cast<uint32_t*>(s.d_ends);
+        cuda_check(launch_token_ends(g, st), "launch(token ends)");
+        if (pipeline_trace()) ch.tr.mark(2, st);
+        cuda_check(cudaEventRecord(cc.kernels, st), "cudaEventRecord");
+        cc.issued = true;
+    };
+    auto stage_c = [&](size_t c) {
+        SChunk& cc = chunks[c];
+        ChunkState& ch = cc.cs;
+        Scratch& s = *lease[c % kDepth]->s;
+        if (!cc.issued) return;
+        cuda_check(cudaEventSynchronize(cc.kernels), "sync(kernels)");
+        const uint64_t ntok = s.h_totals[4];
+        if (tok_total + ntok > token_capacity || (ntok && !token_ends_out)) overflow = true;
+        cudaStream_t so = s.stream_out;
+        cuda_check(cudaStreamWaitEvent(so, cc.kernels, 0), "cudaStreamWaitEvent");
+        if (!overflow) {
+            cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.d_ntok, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
+            cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_st8, ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
+            if (ntok) {
+                cuda_check(cudaMemcpyAsync(token_ends_out + tok_total, s.d_ends, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(ends)");
+                if (tags) {
+                    cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.d_tok, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                    if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.d_cand, ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                }
+            }
+        }
+        cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
+        if (pipeline_trace()) ch.tr.mark(3, so);
+        tok_total += ntok;
+    };
+    // A runs kDepth - 2 chunks ahead of B, B one chunk ahead of C (a scratch is free again when its chunk's C is done)
+    constexpr size_t kAheadA = kDepth - 2;
+    for (size_t c = 0; c < std::min<size_t>(kAheadA, nchunks); ++c) chunk_count(*lease[c % kDepth]->s, chunks[c].cs, utf8, byte_offsets);
+    for (size_t step = 0; step < nchunks + 1; ++step) {
+        if (step + kAheadA < nchunks) chunk_count(*lease[(step + kAheadA) % kDepth]->s, chunks[step + kAheadA].cs, utf8, byte_offsets);
+        if (step < nchunks) stage_b(step);
+        if (step >= 1) stage_c(step - 1);
+    }
+    for (int i = 0; i < kDepth; ++i)
+        if (lease[i]) {
+            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(spans)");
+            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
+        }
+    if (pipeline_trace())
+        for (size_t c = 0; c < nchunks; ++c) chunks[c].cs.tr.print("spans", c, chunks[c].cs.n, chunks[0].cs.tr);
+    if (n_tokens_total_out) *n_tokens_total_out = tok_total;
+    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: token_capacity: too small for the batch");
+    if (want_tags && !tags) std::fill(token_ids_out, token_ids_out + tok_total, -1);  // a model without tag slots
     return kOk;
     VPT_API_END
 }

@@ -200,4 +200,31 @@ struct EvalArgs {
 cudaError_t launch_gold_parse(const EvalArgs& e, cudaStream_t stream);
 cudaError_t launch_eval(const EvalArgs& e, cudaStream_t stream);
 
+// ---- spans.cu: documents -> token byte spans (vaporetto_tantivy's token_stream, vpt_token_spans) --------------------
+struct SpanArgs {
+    const uint8_t* text = nullptr;          // as BatchArgs (offsets absolute; readable up to a multiple of 4 past the end)
+    const uint64_t* offsets = nullptr;      // [n_sent + 1]
+    uint64_t n_sent = 0;
+    const int32_t* status = nullptr;        // from the count pass
+    const uint32_t* n_chars = nullptr;
+    uint8_t* boundaries = nullptr;          // from the scoring pass; 4-byte aligned, readable up to a multiple of 4
+    const uint64_t* bound_offsets = nullptr;  // chunk-local
+    // launch_span_count outputs
+    uint8_t* status8 = nullptr;             // [n_sent]
+    uint32_t* n_tokens = nullptr;           // [n_sent] boundaries set + 1 for a scored document, else 0
+    uint64_t* tok_base = nullptr;           // [n_sent + 1] exclusive prefix of n_tokens, the total behind it
+    uint32_t* tok_local = nullptr;          // [n_sent] scratch: prefix inside a block of kSpanDocs documents
+    uint64_t* tok_blk = nullptr;            // [n_sent / kSpanDocs + 2] scratch: block totals, then their prefix
+    uint64_t* tok_total_host = nullptr;     // nullable: pinned host word that receives the total
+    // launch_token_ends output
+    uint32_t* token_ends = nullptr;         // [total] token r of document s ends at token_ends[tok_base[s] + r]
+};
+constexpr int kSpanDocs = 256;  // documents per block of launch_span_count
+// SplitLinebreaksFilter: the boundary on either side of every '\r' / '\n' becomes 1
+cudaError_t launch_split_linebreaks(const SpanArgs& a, cudaStream_t stream);
+// tokens per document (status8, n_tokens) and their prefix (tok_base)
+cudaError_t launch_span_count(const SpanArgs& a, cudaStream_t stream);
+// the byte offset of every token's exclusive end, relative to its document
+cudaError_t launch_token_ends(const SpanArgs& a, cudaStream_t stream);
+
 }  // namespace vpt
