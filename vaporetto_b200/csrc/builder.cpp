@@ -287,7 +287,10 @@ uint32_t table_slot(const TableGeom& g, const uint8_t* seeds, uint64_t key) {
     key_hashes(key, hash_consts(g.salt), ha, hb);
     const uint32_t bk = bucket_of(ha, g.nbuckets);
     const uint32_t seed = g.seed_bits == 16 ? uint32_t(seeds[2 * size_t(bk)]) | (uint32_t(seeds[2 * size_t(bk) + 1]) << 8) : seeds[bk];
-    return slot_with_seed(ha, hb, seed, g.nslots);
+    // (an 8-bit kSpillSeed only occurs in a table with a spill table, whose geometry follows from g: keys.hpp)
+    if (g.seed_bits != 8 || seed != kSpillSeed) return slot_of_seeds<false>(ha, hb, seed, 0u, g.nslots, 0u, 0u);
+    const uint32_t spill_seed = seeds[spill_bucket_of(hb, g.nbuckets, spill_buckets_of(g.nbuckets))];
+    return slot_of_seeds<true>(ha, hb, seed, spill_seed, g.nslots, spill_slots_of(g.nslots), spill_mul(g.salt));
 }
 
 namespace {
@@ -302,12 +305,53 @@ struct TrieNode {
     uint32_t c1 = 0, c2 = 0, c3 = 0;  // shallow key symbols (depth <= 3)
 };
 
-// Hash-and-displace perfect hash: every bucket of keys gets an 8-bit seed such that all keys land in
-// distinct free slots.  Buckets are placed largest first.
+// Hash-and-displace: gives every bucket of keys the first seed in [0, n_seeds) for which slot(key, seed) sends all
+// its keys to distinct free slots (kSpillSeed is not a placing 8-bit seed).  Buckets are placed largest first.  Returns
+// false when a bucket cannot be placed, unless `spilled` is given: then such a bucket keeps kSpillSeed and its keys
+// are appended to `spilled`.
+template <class SlotF>
+bool place_buckets(const std::vector<std::vector<uint32_t>>& buckets, uint32_t n_seeds, SlotF slot, std::vector<uint8_t>& used,
+                   std::vector<uint32_t>& seed_of_bucket, std::vector<uint32_t>& slot_of_key, std::vector<uint32_t>* spilled) {
+    std::vector<uint32_t> order(buckets.size());
+    std::iota(order.begin(), order.end(), 0u);
+    std::stable_sort(order.begin(), order.end(),
+                     [&](uint32_t a, uint32_t b) { return buckets[a].size() > buckets[b].size(); });
+    seed_of_bucket.assign(buckets.size(), 0);
+    std::vector<uint32_t> tmp;
+    for (uint32_t b : order) {
+        const auto& ks = buckets[b];
+        if (ks.empty()) break;
+        bool placed = false;
+        for (uint32_t seed = 0; seed < n_seeds && !placed; ++seed) {
+            if (n_seeds == 256 && seed == kSpillSeed) continue;
+            tmp.clear();
+            bool ok = true;
+            for (uint32_t ki : ks) {
+                const uint32_t s = slot(ki, seed);
+                if (used[s]) { ok = false; break; }
+                for (uint32_t s2 : tmp) if (s2 == s) { ok = false; break; }
+                if (!ok) break;
+                tmp.push_back(s);
+            }
+            if (ok) {
+                for (size_t k = 0; k < ks.size(); ++k) { used[tmp[k]] = 1; slot_of_key[ks[k]] = tmp[k]; }
+                seed_of_bucket[b] = seed;
+                placed = true;
+            }
+        }
+        if (placed) continue;
+        if (!spilled) return false;
+        seed_of_bucket[b] = kSpillSeed;
+        spilled->insert(spilled->end(), ks.begin(), ks.end());
+    }
+    return true;
+}
+
+// Perfect hash of `keys` with the geometry g (its nslots / nbuckets / salt / seed_bits).  With g.spill (8-bit seeds
+// only), the buckets no seed places go to the spill table (keys.hpp: spill_slots_of ...); g.spill is cleared when none
+// has to.
 bool place_keys(const std::vector<uint64_t>& keys, TableGeom& g, std::vector<uint8_t>& seeds,
                 std::vector<uint32_t>& slot_of_key) {
-    const uint32_t max_seed = g.seed_bits == 16 ? 65536u : 256u;
-    const size_t seed_bytes = g.seed_bits == 16 ? 2 : 1;
     const size_t n = keys.size();
     std::vector<uint32_t> ha(n), hb(n);
     std::vector<std::vector<uint32_t>> buckets(g.nbuckets);
@@ -322,37 +366,34 @@ bool place_keys(const std::vector<uint64_t>& keys, TableGeom& g, std::vector<uin
         std::sort(pairs.begin(), pairs.end());
         if (std::adjacent_find(pairs.begin(), pairs.end()) != pairs.end()) return false;
     }
-    std::vector<uint32_t> order(g.nbuckets);
-    std::iota(order.begin(), order.end(), 0u);
-    std::stable_sort(order.begin(), order.end(),
-                     [&](uint32_t a, uint32_t b) { return buckets[a].size() > buckets[b].size(); });
     std::vector<uint8_t> used(g.nslots, 0);
-    seeds.assign(size_t(g.nbuckets) * seed_bytes, 0);
+    std::vector<uint32_t> seed_of_bucket, spilled;
     slot_of_key.assign(n, 0);
-    std::vector<uint32_t> tmp;
-    for (uint32_t b : order) {
-        const auto& ks = buckets[b];
-        if (ks.empty()) break;
-        bool placed = false;
-        for (uint32_t seed = 0; seed < max_seed && !placed; ++seed) {
-            tmp.clear();
-            bool ok = true;
-            for (uint32_t ki : ks) {
-                const uint32_t slot = slot_with_seed(ha[ki], hb[ki], seed, g.nslots);
-                if (used[slot]) { ok = false; break; }
-                for (uint32_t s2 : tmp) if (s2 == slot) { ok = false; break; }
-                if (!ok) break;
-                tmp.push_back(slot);
-            }
-            if (ok) {
-                for (size_t k = 0; k < ks.size(); ++k) { used[tmp[k]] = 1; slot_of_key[ks[k]] = tmp[k]; }
-                if (seed_bytes == 2) { seeds[2 * size_t(b)] = uint8_t(seed); seeds[2 * size_t(b) + 1] = uint8_t(seed >> 8); }
-                else seeds[b] = uint8_t(seed);
-                placed = true;
-            }
-        }
-        if (!placed) return false;
+    const auto primary = [&](uint32_t ki, uint32_t seed) { return slot_of_seeds<false>(ha[ki], hb[ki], seed, 0, g.nslots, 0, 0); };
+    if (!place_buckets(buckets, g.seed_bits == 16 ? 65536u : 256u, primary, used, seed_of_bucket, slot_of_key,
+                       g.spill ? &spilled : nullptr))
+        return false;
+    g.spill = !spilled.empty();
+    std::vector<uint32_t> spill_seeds;
+    if (g.spill) {
+        const uint32_t nsb = spill_buckets_of(g.nbuckets), nss = spill_slots_of(g.nslots), mul = spill_mul(g.salt);
+        std::vector<std::vector<uint32_t>> sb(nsb);
+        for (uint32_t ki : spilled) sb[spill_bucket_of(hb[ki], 0, nsb)].push_back(ki);
+        std::vector<uint8_t> sused(nss, 0);
+        const auto spill = [&](uint32_t ki, uint32_t seed) {
+            return slot_of_seeds<true>(ha[ki], hb[ki], kSpillSeed, seed, g.nslots, nss, mul) - g.nslots;
+        };
+        std::vector<uint32_t> sk(slot_of_key);
+        if (!place_buckets(sb, 256u, spill, sused, spill_seeds, sk, nullptr)) return false;
+        for (uint32_t ki : spilled) slot_of_key[ki] = sk[ki] + g.nslots;
     }
+    const size_t seed_bytes = g.seed_bits == 16 ? 2 : 1;
+    seeds.assign(size_t(g.nbuckets) * seed_bytes + spill_seeds.size(), 0);
+    for (size_t b = 0; b < g.nbuckets; ++b) {
+        seeds[seed_bytes * b] = uint8_t(seed_of_bucket[b]);
+        if (seed_bytes == 2) seeds[2 * b + 1] = uint8_t(seed_of_bucket[b] >> 8);
+    }
+    for (size_t b = 0; b < spill_seeds.size(); ++b) seeds[g.nbuckets + b] = uint8_t(spill_seeds[b]);
     return true;
 }
 
@@ -438,9 +479,25 @@ NodeTable build_node_table(const PatternSet& ps, bool force_general, uint32_t bu
     // on failure retry with another salt and a sparser table, then with smaller buckets.
     static const double kAlpha[] = {0.60, 0.50, 0.42, 0.35, 0.30, 0.30, 0.25, 0.25, 0.20, 0.15};
     static const double kLambda[] = {8.0, 8.0, 8.0, 8.0, 8.0, 6.0, 6.0, 4.0, 4.0, 3.0};
+    // Inline-format tables whose seeds fit the shared-memory budget are built dense: load 0.75 in the primary slots,
+    // and the buckets no seed places there go to a small sparse spill table whose seeds share the budget (keys.hpp).
+    // A probe is still one seed pair and one record load; the records take about a third less L2 than a sparse
+    // table's, and L2 is what the probes are served from (DESIGN.md §4).
+    if (t.fast && bucket_cap) {
+        // (9 keys per primary bucket leave room in the budget for the spill seeds; config 2: 15 % of the keys spill)
+        static const double kDenseLambda[] = {9.0, 9.0, 9.5};
+        for (int attempt = 0; attempt < 3 && !ok; ++attempt) {
+            t.geom.nslots = uint32_t(std::max<double>(16.0, double(n) / 0.75 + 1.0));
+            t.geom.nbuckets = uint32_t(std::max<double>(1.0, double(n) / kDenseLambda[attempt] + 1.0));
+            t.geom.salt = 0x3c6ef372fe94f82bULL * uint64_t(attempt + 1);
+            t.geom.spill = true;
+            if (t.geom.nbuckets + spill_buckets_of(t.geom.nbuckets) <= bucket_cap) ok = place_keys(keys, t.geom, t.seeds, slot_of_key);
+        }
+        if (!ok) t.geom.spill = false;
+    }
     // Tables slightly too large for the kernel's shared seed buffer first try fatter buckets (<= 12 keys) on a
     // sparse table so that the seeds still fit.
-    if (bucket_cap && double(n) / 8.0 + 1.0 > double(bucket_cap) && double(n) / 12.0 < double(bucket_cap)) {
+    if (!ok && bucket_cap && double(n) / 8.0 + 1.0 > double(bucket_cap) && double(n) / 12.0 < double(bucket_cap)) {
         for (int attempt = 0; attempt < 2 && !ok; ++attempt) {
             t.geom.nslots = uint32_t(double(n) / (attempt ? 0.25 : 0.33) + 1.0);
             t.geom.nbuckets = bucket_cap;
@@ -450,7 +507,7 @@ NodeTable build_node_table(const PatternSet& ps, bool force_general, uint32_t bu
     }
     // Tables far beyond the shared-memory seed budget are built dense instead (16-bit seeds, load factor 0.85):
     // what matters for them is staying resident in L2.
-    if (bucket_cap && double(n) / 12.0 >= double(bucket_cap)) {
+    if (!ok && bucket_cap && double(n) / 12.0 >= double(bucket_cap)) {
         static const double kDenseAlpha[] = {0.85, 0.80, 0.70};
         for (int attempt = 0; attempt < 3 && !ok; ++attempt) {
             t.geom.seed_bits = 16;
@@ -470,12 +527,13 @@ NodeTable build_node_table(const PatternSet& ps, bool force_general, uint32_t bu
     if (!ok) throw Error(kInternal, "internal error: perfect hash construction failed");
 
     // 4. records
-    t.records.assign(size_t(t.geom.nslots) * 32, 0);
-    t.slot_node.assign(t.geom.nslots, 0);
-    t.slot_pid.assign(t.geom.nslots, kNoPattern);
+    const size_t total_slots = size_t(t.geom.nslots) + (t.geom.spill ? spill_slots_of(t.geom.nslots) : 0u);
+    t.records.assign(total_slots * 32, 0);
+    t.slot_node.assign(total_slots, 0);
+    t.slot_pid.assign(total_slots, kNoPattern);
     std::vector<uint32_t> ovf_ptr;
     if (t.has_overflow) {
-        t.slot_ovf.assign(t.geom.nslots, 0);
+        t.slot_ovf.assign(total_slots, 0);
         ovf_ptr.assign(ps.rows.size(), kNoPattern);
         for (const auto& r : ps.rows)
             if (r.w.size() > 65535) throw Error(kInvalidModel, "InvalidModelError: weight row too long");

@@ -52,12 +52,13 @@ struct NodeTable {
     TableGeom geom;
     uint32_t n_nodes = 0;
     uint32_t max_depth = 0;
-    std::vector<uint8_t> records;       // nslots * 32 bytes
-    std::vector<uint8_t> seeds;         // nbuckets
-    std::vector<uint32_t> slot_node;    // nslots: node id of the record in the slot (deep keys)
-    std::vector<uint32_t> slot_pid;     // nslots: best pattern id (tag states); fast tables only
+    std::vector<uint8_t> records;       // (nslots + spill_slots) * 32 bytes
+    std::vector<uint8_t> seeds;         // nbuckets (x 2 for 16-bit seeds), then spill_buckets
+    std::vector<uint32_t> slot_node;    // per slot: node id of the record in the slot (deep keys)
+    std::vector<uint32_t> slot_pid;     // per slot: best pattern id (tag states); fast tables only
     std::vector<int32_t> pool;          // general rows / overflow rows (full row with the inline part zeroed)
     std::vector<uint64_t> slot_ovf;     // fast tables with overflow: ptr | (off & 0xFFFF) << 32 | len << 48 per slot
+                                        // (the spill slots follow the primary ones in all four per-slot arrays)
     bool has_overflow = false;
     int rel_min = 0, rel_max = 0;       // union extent of all rows: [rel_min, rel_max)
 };

@@ -171,6 +171,9 @@ DevTable dev_table(const BlobTable& bt, const uint8_t* base) {
     d.salt = bt.salt;
     d.hk = hash_consts(bt.salt);
     d.seed16 = bt.seed_bits == 16;
+    d.spill_slots = bt.spill_slots;
+    d.spill_buckets = bt.spill_buckets;
+    d.spill_mul = spill_mul(bt.salt);
     d.has_overflow = bt.has_overflow;
     d.slot_ovf = bt.has_overflow ? reinterpret_cast<const uint64_t*>(base + bt.ovf_off) : nullptr;
     d.records = base + bt.rec_off;
@@ -183,16 +186,25 @@ DevTable dev_table(const BlobTable& bt, const uint8_t* base) {
 
 // Every section a blob header points at must lie inside the blob, and the geometry must be what the kernels were
 // built for: a truncated or corrupted blob is an InvalidModel error, not an out-of-bounds read on the device.
-void validate_blob_header(const BlobHeader& h, uint64_t len) {
+void validate_blob_header(const BlobHeader& h, const uint8_t* base, uint64_t len) {
     auto inside = [&](uint64_t off, uint64_t bytes) { return off >= sizeof(BlobHeader) && off <= len && bytes <= len - off; };
     auto bad = [](const char* what) { return Error(kInvalidModel, std::string("InvalidModelError: model blob: bad ") + what); };
     auto table = [&](const BlobTable& t, const char* name) {
         if (!t.present) return;
         if (t.nslots == 0 || t.nbuckets == 0 || (t.seed_bits != 8 && t.seed_bits != 16)) throw bad(name);
-        if (!inside(t.rec_off, uint64_t(t.nslots) * 32) || !inside(t.seeds_off, uint64_t(t.nbuckets) * (t.seed_bits / 8)) ||
-            !inside(t.node_off, uint64_t(t.nslots) * 4) || !inside(t.pid_off, uint64_t(t.nslots) * 4) || !inside(t.pool_off, 4))
+        // a spill table needs 8-bit seeds that k_fused stages in shared memory, where it reads the spill seeds
+        if ((t.spill_slots || t.spill_buckets) &&
+            (t.spill_slots != spill_slots_of(t.nslots) || t.spill_buckets != spill_buckets_of(t.nbuckets) || t.seed_bits != 8 ||
+             uint64_t(t.nbuckets) + t.spill_buckets > uint64_t(fused_detail::kSeedCap)))
             throw bad(name);
-        if (t.has_overflow && !inside(t.ovf_off, uint64_t(t.nslots) * 8)) throw bad(name);
+        const uint64_t slots = uint64_t(t.nslots) + t.spill_slots;
+        const uint64_t seed_bytes = uint64_t(t.nbuckets) * (t.seed_bits / 8) + t.spill_buckets;
+        if (slots > 0xFFFFFFFFull || !inside(t.rec_off, slots * 32) || !inside(t.seeds_off, seed_bytes) ||
+            !inside(t.node_off, slots * 4) || !inside(t.pid_off, slots * 4) || !inside(t.pool_off, 4))
+            throw bad(name);
+        if (t.has_overflow && !inside(t.ovf_off, slots * 8)) throw bad(name);
+        // an 8-bit table without a spill table carries no spill seed (its probes would land behind the records)
+        if (t.seed_bits == 8 && !t.spill_slots && memchr(base + t.seeds_off, int(kSpillSeed), t.nbuckets)) throw bad(name);
         if (t.r0 < -64 || t.r0 > 64) throw bad(name);
     };
     table(h.ct, "char table");
@@ -630,7 +642,7 @@ int vpt_predictor_from_blob(const void* blob, uint64_t len, int device, vpt_pred
     memcpy(&h, blob, sizeof h);
     if (memcmp(h.magic, kBlobMagic, 8) != 0 || h.total_bytes != len)
         throw Error(kInvalidModel, "InvalidModelError: not a vaporetto_b200 model blob");
-    validate_blob_header(h, len);
+    validate_blob_header(h, static_cast<const uint8_t*>(blob), len);
     std::unique_ptr<vpt_predictor> p(new vpt_predictor());
     p->device = device;
     p->from_blob = true;

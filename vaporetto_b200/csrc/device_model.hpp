@@ -20,6 +20,9 @@ struct DevTable {
     HashK hk{};                        // hash multipliers derived from the salt (keys.hpp)
     uint32_t nslots = 0;
     uint32_t nbuckets = 0;
+    uint32_t spill_slots = 0;          // spill table (keys.hpp: slot_of_seeds); its seeds follow the nbuckets ones
+    uint32_t spill_buckets = 0;
+    uint32_t spill_mul = 0;
     int32_t r0 = 0;
     uint32_t max_depth = 0;
     int32_t present = 0;

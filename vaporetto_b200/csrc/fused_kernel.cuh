@@ -276,6 +276,7 @@ __device__ __forceinline__ void zero_sentence(const BatchArgs& a, uint64_t ob, u
 // ---- rare paths of the stream stage -----------------------------------------------------------------------------------
 
 // Continues a 3-character hit backwards through the slot stream for patterns longer than three characters.
+template <bool kSeedsSmem>
 __device__ __forceinline__ bool deep_walk_f(const DevTable& t, const uint32_t* s_raw, int p, bool norm, uint32_t& slot, Rec32& rec) {
     bool deep_hit = false;
     uint32_t node = __ldg(t.slot_node + slot);
@@ -287,7 +288,7 @@ __device__ __forceinline__ bool deep_walk_f(const DevTable& t, const uint32_t* s
         uint32_t c = decode_any(x, bad, len);  // (not the warp-wide decoder: only some lanes walk)
         if (norm) c = kytea_fullwidth(c);
         const uint64_t key = deep_key(node, c);
-        const uint32_t nslot = slot_of(t, key);
+        const uint32_t nslot = slot_of<kSeedsSmem>(t, key);
         const Rec32 nrec = load_record(t.records, nslot);
         const uint64_t k = (uint64_t(nrec.v[1]) << 32) | nrec.v[0];
         if ((k & ~(kExtFlag | kOvfFlag)) != key) break;
@@ -329,14 +330,16 @@ __device__ __forceinline__ uint32_t seed_of(const DevTable& t, const uint8_t* s_
                       : t.seed16 ? uint32_t(__ldg(reinterpret_cast<const uint16_t*>(t.seeds) + b)) : uint32_t(__ldg(t.seeds + b));
 }
 
-// Slot of `key hashes (h, g)` in the node table, and its record.
+// Slot of `key hashes (h, g)` in the node table, and its record.  The spill seed is read beside the primary one (no
+// dependent load); only tables whose seeds are staged in shared memory have a spill table (validate_blob_header).
 template <bool kSeedsSmem>
 __device__ __forceinline__ Rec32 probe_load(const DevTable& ct, const uint8_t* s_seeds, uint32_t h, uint32_t g, uint32_t& slot) {
     const uint32_t seed = seed_of<kSeedsSmem>(ct, s_seeds, mulhi32(h, ct.nbuckets));
-    // (as PTX: the compiler otherwise folds "high word of the product, times 32" into a 64-bit shift/mask sequence of six
-    //  ALU-pipe instructions; this is IMAD.HI + IMAD.WIDE on the FMA pipe -- the kernel's ALU pipe is its busiest unit)
+    const uint32_t spill_seed = kSeedsSmem ? uint32_t(s_seeds[spill_bucket_of(g, ct.nbuckets, ct.spill_buckets)]) : 0u;
+    slot = slot_of_seeds<kSeedsSmem>(h, g, seed, spill_seed, ct.nslots, ct.spill_slots, ct.spill_mul);
+    // (as PTX: the compiler otherwise folds "slot times 32" into a 64-bit shift/mask sequence of ALU-pipe instructions;
+    //  this is IMAD.WIDE on the FMA pipe -- the kernel's ALU pipe is its busiest unit)
     uint64_t addr;
-    asm("mul.hi.u32 %0, %1, %2;" : "=r"(slot) : "r"((g + seed * (h | 1u)) * 0x85EBCA6Bu), "r"(ct.nslots));
     asm("mad.wide.u32 %0, %1, 32, %2;" : "=l"(addr) : "r"(slot), "l"(ct.records));
     return load_record(reinterpret_cast<const void*>(addr), 0);
 }
@@ -395,7 +398,7 @@ __device__ __forceinline__ void stream_stage(const DevModel& m, const BatchArgs&
             if (kDeep > 0) {
                 if (f2 && (flB & 4u) && (rB.v[1] >> 31)) {
                     // a 3-character node with longer extensions: walk on (patterns longer than 3: dictionary words)
-                    const bool dh = deep_walk_f(ct, s_raw, p, cfg.norm, slB, rB);
+                    const bool dh = deep_walk_f<kSeedsSmem>(ct, s_raw, p, cfg.norm, slB, rB);
                     // (the slots of the halo and behind the range end are walked by two warps: only the owner adds)
                     if (kOverflow) { if (dh && (rB.v[1] & (1u << 29)) && p >= ra && p < rb) apply_overflow_f(ct, slB, p, s_raw, s_acc); }
                 }
@@ -552,7 +555,7 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
 
     // ---- CTA-shared tables -------------------------------------------------------------------------------------
     if (kSeedsSmem) {
-        const uint32_t nwords = (m.ct.nbuckets + 3) / 4;
+        const uint32_t nwords = (m.ct.nbuckets + m.ct.spill_buckets + 3) / 4;
         const uint32_t* src = reinterpret_cast<const uint32_t*>(m.ct.seeds);
         for (uint32_t i = threadIdx.x; i < nwords; i += Lay::kThreads) reinterpret_cast<uint32_t*>(s_seeds)[i] = __ldg(src + i);
     }

@@ -52,7 +52,7 @@ constexpr int kTileSubBlocks = 4;
 inline bool inline_rows(const DevModel& m) { return (!m.ct.present || m.ct.fast) && !m.tt.present; }
 
 inline bool seeds_smem(const DevModel& m) {
-    return m.ct.present && !m.ct.seed16 && m.ct.nbuckets <= uint32_t(fused_detail::kSeedCap);
+    return m.ct.present && !m.ct.seed16 && m.ct.nbuckets + m.ct.spill_buckets <= uint32_t(fused_detail::kSeedCap);
 }
 
 // separator slots between the sentences of a tile, so that neither the weight-row gather (window [r0, r0 + 6)) nor the

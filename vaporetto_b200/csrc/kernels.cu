@@ -412,7 +412,12 @@ __device__ __forceinline__ uint32_t slot_of_t(const DevTable& t, const uint8_t* 
     const uint32_t seed = kSeedsSmem ? uint32_t(s_seeds[b])
                                      : t.seed16 ? uint32_t(__ldg(reinterpret_cast<const uint16_t*>(t.seeds) + b))
                                                 : uint32_t(__ldg(t.seeds + b));
-    return slot_with_seed(ha, hb, seed, t.nslots);
+    // (staged seeds: read the spill seed unconditionally, beside the primary one; index nbuckets, in the buffer, without
+    //  a spill table)
+    const uint32_t sb = spill_bucket_of(hb, t.nbuckets, t.spill_buckets);
+    if (kSeedsSmem) return slot_of_seeds<true>(ha, hb, seed, uint32_t(s_seeds[sb]), t.nslots, t.spill_slots, t.spill_mul);
+    if (!t.spill_buckets) return slot_of_seeds<false>(ha, hb, seed, 0u, t.nslots, 0u, 0u);
+    return slot_of_seeds<true>(ha, hb, seed, uint32_t(__ldg(t.seeds + sb)), t.nslots, t.spill_slots, t.spill_mul);
 }
 
 __device__ __forceinline__ bool rec_matches(const Rec32& rec, uint64_t key) {
@@ -555,7 +560,7 @@ __global__ void __launch_bounds__(kTileThreads, 1) k_tile_fast(DevModel m, Batch
     // ---- CTA-shared tables ----------------------------------------------------------------------------
     const bool tsplit = kSplit3;
     if (kSeedsSmem) {
-        const uint32_t nwords = (m.ct.nbuckets + 3) / 4;
+        const uint32_t nwords = (m.ct.nbuckets + m.ct.spill_buckets + 3) / 4;
         const uint32_t* src = reinterpret_cast<const uint32_t*>(m.ct.seeds);
         for (uint32_t i = threadIdx.x; i < nwords; i += kTileThreads) reinterpret_cast<uint32_t*>(s_seeds)[i] = __ldg(src + i);
     }

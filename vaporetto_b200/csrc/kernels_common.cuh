@@ -53,12 +53,17 @@ __device__ __forceinline__ Rec32 load_record(const void* base, uint32_t slot) {
     return r;
 }
 
+// kMaySpill = false: the caller knows the table has no spill table (its seeds are not staged in shared memory:
+// validate_blob_header)
+template <bool kMaySpill = true>
 __device__ __forceinline__ uint32_t slot_of(const DevTable& t, uint64_t key) {
     uint32_t ha, hb;
     key_hashes(key, t.hk, ha, hb);
     const uint32_t b = bucket_of(ha, t.nbuckets);
     const uint32_t seed = t.seed16 ? uint32_t(__ldg(reinterpret_cast<const uint16_t*>(t.seeds) + b)) : uint32_t(__ldg(t.seeds + b));
-    return slot_with_seed(ha, hb, seed, t.nslots);
+    if (!kMaySpill || !t.spill_buckets) return slot_of_seeds<false>(ha, hb, seed, 0u, t.nslots, 0u, 0u);
+    const uint32_t spill_seed = __ldg(t.seeds + spill_bucket_of(hb, t.nbuckets, t.spill_buckets));
+    return slot_of_seeds<true>(ha, hb, seed, spill_seed, t.nslots, t.spill_slots, t.spill_mul);
 }
 
 // One probe: returns true when the node with `key` exists; rec/slot are valid then.

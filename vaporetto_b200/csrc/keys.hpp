@@ -9,12 +9,16 @@ namespace vpt {
 constexpr uint32_t kNoPattern = 0xFFFFFFFFu;
 constexpr int kInlineWidth = 6;  // weights stored inside a 32-byte fast record
 
-// Hash-table geometry shared by host builder and device kernels.
+// Hash-table geometry shared by host builder and device kernels.  A dense table with 8-bit seeds places most keys in
+// its nslots primary slots; the buckets no seed could place there carry kSpillSeed, and their keys live in a sparse
+// spill table behind the primary ones (one slot space: slot numbers nslots .. nslots + spill_slots_of(nslots) - 1),
+// whose spill_buckets_of(nbuckets) seeds follow the nbuckets primary seeds.
 struct TableGeom {
     uint32_t nslots = 0;
     uint32_t nbuckets = 0;
     uint64_t salt = 0;
     uint32_t seed_bits = 8;  // 8: one byte per bucket (fits shared memory); 16: dense tables that live in L2
+    bool spill = false;      // the table has a spill table (8-bit seeds only)
 };
 
 // 32-byte records.  `key` bit 63 = node has longer extensions (a deeper node exists).
@@ -81,12 +85,41 @@ VPT_HD void key_hashes(uint64_t key, const HashK& k, uint32_t& ha, uint32_t& hb)
     ha = c3 * k.a[0] + c2 * k.a[1] + c1 * k.a[2];
     hb = c3 * k.b[0] + c2 * k.b[1] + c1 * k.b[2];
 }
-VPT_HD uint32_t mulhi32(uint32_t a, uint32_t b) { return uint32_t((uint64_t(a) * b) >> 32); }
+VPT_HD uint32_t mulhi32(uint32_t a, uint32_t b) {
+#ifdef __CUDA_ARCH__
+    return __umulhi(a, b);  // one IMAD.HI (the 64-bit form can become a wide product and a shift)
+#else
+    return uint32_t((uint64_t(a) * b) >> 32);
+#endif
+}
 VPT_HD uint32_t child_bit(uint32_t c1) { return mulhi32(c1 * 0x9E3779B1u, uint32_t(kChildMaskBits)); }
 VPT_HD uint32_t bucket_of(uint32_t ha, uint32_t nbuckets) { return mulhi32(ha, nbuckets); }
-VPT_HD uint32_t slot_with_seed(uint32_t ha, uint32_t hb, uint32_t seed, uint32_t nslots) {
-    const uint32_t v = (hb + seed * (ha | 1u)) * 0x85EBCA6Bu;
-    return mulhi32(v, nslots);
+// The probe rule: key hashes + seeds -> slot.  In a table with a spill table, a primary seed of kSpillSeed (never a
+// placing 8-bit seed) sends the key to the spill table: its bucket there is picked by the displacement hash hb
+// (spill_bucket_of), it is displaced by kSpillSeed + that bucket's seed with the spill table's own multiplier, into
+// slots nslots ...  Both seeds are read before this (the spill seed whether it is needed or not, so that the two
+// loads are independent); the spill seed only counts for a spilled bucket.  kSpill = false is the rule of a table
+// without a spill table (every seed places; 16-bit seeds); an 8-bit table without one never carries kSpillSeed, so
+// kSpill = true serves it too.  The selects are multiply-adds by sp (0 / 1): the kernels' ALU pipe is their busiest
+// unit, the FMA pipe is not.
+constexpr uint32_t kSpillSeed = 255;
+constexpr uint32_t kPrimaryMul = 0x85EBCA6Bu;
+// The spill table's geometry follows from the primary one, so that nslots, nbuckets, the salt and the seeds are all a
+// prober needs: a third as many slots (about 18 % of a 0.75-load table's keys spill: load ~0.35), an eighth as many
+// buckets (8-12 keys each), and a displacement multiplier of its own derived from the salt.
+VPT_HD uint32_t spill_slots_of(uint32_t nslots) { return nslots / 3 + 1; }
+VPT_HD uint32_t spill_buckets_of(uint32_t nbuckets) { return nbuckets / 8 + 1; }
+VPT_HD uint32_t spill_mul(uint64_t salt) { return uint32_t(mix64(salt + 0x9E3779B97F4A7C15ull * 4)) | 1u; }
+// index of a key's spill seed in the seed array (the spill seeds follow the nbuckets primary ones)
+VPT_HD uint32_t spill_bucket_of(uint32_t hb, uint32_t nbuckets, uint32_t spill_buckets) {
+    return mulhi32(hb, spill_buckets) + nbuckets;
+}
+template <bool kSpill>
+VPT_HD uint32_t slot_of_seeds(uint32_t ha, uint32_t hb, uint32_t seed, uint32_t spill_seed, uint32_t nslots,
+                              uint32_t spill_slots, uint32_t spill_multiplier) {
+    const uint32_t sp = kSpill && seed == kSpillSeed ? 1u : 0u;
+    const uint32_t v = (hb + (seed + sp * spill_seed) * (ha | 1u)) * (kPrimaryMul + sp * (spill_multiplier - kPrimaryMul));
+    return mulhi32(v, nslots + sp * (spill_slots - nslots)) + sp * nslots;
 }
 
 }  // namespace vpt

@@ -31,6 +31,8 @@ void write_table(BlobWriter& w, const NodeTable& t, size_t n_patterns, BlobTable
     bt.nbuckets = t.geom.nbuckets;
     bt.salt = t.geom.salt;
     bt.seed_bits = t.geom.seed_bits;
+    bt.spill_slots = t.geom.spill ? spill_slots_of(t.geom.nslots) : 0u;
+    bt.spill_buckets = t.geom.spill ? spill_buckets_of(t.geom.nbuckets) : 0u;
     bt.n_nodes = t.n_nodes;
     bt.n_patterns = uint32_t(n_patterns);
     bt.rec_off = w.add(t.records.data(), t.records.size());

@@ -11,7 +11,7 @@
 
 namespace vpt {
 
-constexpr char kBlobMagic[8] = {'V', 'P', 'T', 'B', '2', '0', '0', '\5'};
+constexpr char kBlobMagic[8] = {'V', 'P', 'T', 'B', '2', '0', '0', '\6'};
 
 struct BlobTable {
     uint64_t rec_off, seeds_off, node_off, pid_off, pool_off;
@@ -23,6 +23,9 @@ struct BlobTable {
     uint32_t n_nodes, n_patterns;
     uint32_t seed_bits, has_overflow;
     uint64_t ovf_off;
+    // spill table (keys.hpp: spill_slots_of / spill_buckets_of of the primary geometry): its records and side-array
+    // entries follow the nslots primary ones, its seeds the nbuckets primary ones; 0 / 0 = none
+    uint32_t spill_slots, spill_buckets;
 };
 struct BlobHeader {
     char magic[8];
