@@ -3,11 +3,9 @@
 #include "../../include/vaporetto_b200.h"
 
 #include <algorithm>
-#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <deque>
 #include <functional>
 #include <memory>
 #include <mutex>
@@ -975,21 +973,30 @@ size_t chunk_bytes() {
 constexpr uint64_t kMaxLineChunk = uint64_t(1) << 30;  // 32-bit group-local output offsets (3 bytes out per byte in)
 
 struct LineChunk {
-    uint64_t byte_lo = 0, nbytes = 0;
+    uint64_t nbytes = 0;
     uint64_t n_lines = 0;
     cudaEvent_t split = nullptr, done = nullptr;
     TraceEvents tr;
     SplitArgs sp;
 };
 
-// stage 0 of a chunk: H2D of the text, newline counts, the number of lines to pinned host memory
-void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* utf8) {
+// What a line loop computes: the flags of vpt_tokenize_lines*, vpt_evaluate_lines or vpt_line_stream_new, checked
+struct LineJob {
+    int kind;          // VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE
+    bool normalize;    // KyteaFullwidthFilter (no_norm == 0)
+    uint32_t wsconst;  // post-filters (VPT_WSCONST_*)
+    bool tags;         // tags predicted on the device
+    int tag_mode;      // evaluate: how the system's tags compare with the gold's (kTags*)
+};
+
+// stage 0 of a chunk: H2D of its `nbytes` at `bytes`, newline counts, the number of lines to pinned host memory
+void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* bytes) {
     cudaStream_t st = s.stream;
     const size_t nblk = (ch.nbytes + kSplitBlockBytes - 1) / kSplitBlockBytes;
     Scratch::ensure(s.d_text, s.text_cap, ch.nbytes + 64);
     Scratch::ensure(s.d_blk, s.blk_cap, 4 * nblk + 4);
     Scratch::ensure(s.d_blkbase, s.blkbase_cap, 8 * nblk + 16);
-    cuda_check(cudaMemcpyAsync(s.d_text, utf8 + ch.byte_lo, ch.nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
+    cuda_check(cudaMemcpyAsync(s.d_text, bytes, ch.nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
     if (pipeline_trace()) ch.tr.mark(0, st);
     SplitArgs& sp = ch.sp;
     sp = SplitArgs();
@@ -1005,11 +1012,11 @@ void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* utf8) {
 }
 
 // Scores the sentences of `a` (text, offsets, trims, n_sent set; `nbytes` bounds their bytes), runs the --wsconst
-// post-filters and, with `tags`, predicts the tags of every token into per-token records (the post-filters ran first:
-// fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
+// post-filters and, with `job.tags`, predicts the tags of every token into per-token records (the post-filters ran
+// first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
 // records; its output fields are left to the caller.
-TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, bool normalize,
-                      uint32_t wsconst, bool tags) {
+TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job) {
+    const bool normalize = job.normalize, tags = job.tags;
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
     const WorkspaceLayout wl = workspace_layout(n);
@@ -1052,8 +1059,8 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     t.n_chars = a.n_chars;
     t.boundaries = a.boundaries;
     t.bound_offsets = a.bound_offsets;
-    cuda_check(launch_wsconst(t, a.boundaries, wsconst, normalize, st), "launch(wsconst)");
-    if (wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
+    cuda_check(launch_wsconst(t, a.boundaries, job.wsconst, normalize, st), "launch(wsconst)");
+    if (job.wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
     if (tags) {
         // tokens per sentence and their prefix, then the tag prediction into per-token records
         CompactArgs k;
@@ -1109,34 +1116,44 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     return t;
 }
 
-// stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
-void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normalize, uint32_t wsconst, bool tags) {
+// The start of stage 1, for tokenize and evaluate alike: waits for the chunk's line count and, when it has lines, writes
+// their offsets and trims.  Returns the line count; the chunk's `done` event exists on return.
+size_t split_lines(Scratch& s, LineChunk& ch) {
     cudaStream_t st = s.stream;
     cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
     const size_t n = size_t(s.h_totals[2]);
     ch.n_lines = n;
     if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
-    s.h_totals[3] = 0;
-    if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
+    if (n == 0) return 0;
     const size_t ng = (n + kGroup - 1) / kGroup;
     Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
     Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
     Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
-    // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
-    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
-    Scratch::ensure(s.d_out, s.out_cap, 3 * ch.nbytes + n + 4 + (tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0));
     ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
     ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
-    // the kernels overwrite d_out, which the previous chunk of this scratch may still be copying out
+    // the kernels of the stage overwrite outputs (d_out, d_lc) the previous chunk of this scratch may still be copying out
     cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
     if (pipeline_trace()) ch.tr.mark(1, st);
     cuda_check(launch_split_write(ch.sp, st), "launch(split)");
+    return n;
+}
+
+// stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
+void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
+    cudaStream_t st = s.stream;
+    const size_t n = split_lines(s, ch);
+    s.h_totals[3] = 0;
+    if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
+    const size_t ng = (n + kGroup - 1) / kGroup;
+    // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
+    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
+    Scratch::ensure(s.d_out, s.out_cap, 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0));
     BatchArgs a;
     a.text = ch.sp.text;
     a.offsets = ch.sp.offsets;
     a.trims = ch.sp.trims;
     a.n_sent = n;
-    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, normalize, wsconst, tags);
+    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job);
     t.tok_state = static_cast<uint64_t*>(s.d_tokg);
     t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
     t.total = t.tok_state + ng + 1;
@@ -1168,12 +1185,19 @@ bool check_lines_flags(const vpt_predictor* p, uint32_t wsconst_types, bool tags
     return tags;
 }
 
+LineJob line_job(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst_types, bool predict_tags) {
+    const bool tags = check_lines_flags(p, wsconst_types, predict_tags);
+    // main.rs:110-120 with predictor.rs:553: the system keeps the gold tags (--no-norm) or has none, unless tags are
+    // predicted with a model that has tag slots
+    return {kind, no_norm == 0, wsconst_types, tags, tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty};
+}
+
 // Cuts a buffer of lines into pipeline chunks that end after a '\n' (memrchr from the nominal cut; a line longer than a
-// chunk extends it to the line's end)
-std::vector<LineChunk> line_chunks(const uint8_t* utf8, size_t n_bytes) {
+// chunk extends it to the line's end); returns the end of every chunk
+std::vector<size_t> line_chunks(const uint8_t* utf8, size_t n_bytes) {
     const size_t big = chunk_bytes();
     const std::vector<size_t> sizes = ramp_schedule(n_bytes, big, big / 8, big / 8);
-    std::vector<LineChunk> chunks;
+    std::vector<size_t> ends;
     size_t cum = 0, k = 0;
     for (size_t lo = 0; lo < n_bytes;) {
         // every chunk ends at the next nominal cut of the schedule (a line that ran past cuts skips them)
@@ -1188,107 +1212,19 @@ std::vector<LineChunk> line_chunks(const uint8_t* utf8, size_t n_bytes) {
             }
         }
         if (hi - lo > kMaxLineChunk) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: a line is longer than 1 GiB");
-        LineChunk ch;
-        ch.byte_lo = lo;
-        ch.nbytes = hi - lo;
-        chunks.push_back(ch);
+        ends.push_back(hi);
         lo = hi;
     }
-    return chunks;
+    return ends;
 }
-
-int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
-                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
-    VPT_API_BEGIN
-    tags = check_lines_flags(p, wsconst_types, tags);
-    if (out_len) *out_len = 0;
-    if (n_lines_out) *n_lines_out = 0;
-    if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
-    if (n_bytes == 0) return kOk;
-    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-
-    std::vector<LineChunk> chunks = line_chunks(utf8, n_bytes);
-    const size_t nchunks = chunks.size();
-    constexpr int kDepth = 4;
-    std::unique_ptr<ScratchLease> lease[kDepth];
-    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
-    struct EventGuard {
-        std::vector<LineChunk>& c;
-        ~EventGuard() {
-            for (auto& x : c) {
-                if (x.split) cudaEventDestroy(x.split);
-                if (x.done) cudaEventDestroy(x.done);
-                x.tr.destroy();
-            }
-        }
-    } guard{chunks};
-
-    // chunks c+2, c+3 are copied in and split while chunk c+1 is scored and chunk c is copied out
-    uint64_t total = 0, lines = 0;
-    bool overflow = false;
-    const bool trace = pipeline_trace();
-    const auto host_t0 = std::chrono::steady_clock::now();
-    auto host_ms = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count(); };
-    for (size_t c = 0; c < std::min<size_t>(3, nchunks); ++c) lines_stage0(*lease[c % kDepth]->s, chunks[c], utf8);
-    lines_stage1(*p, *lease[0]->s, chunks[0], no_norm == 0, wsconst_types, tags);
-    for (size_t c = 0; c < nchunks; ++c) {
-        const double h0 = host_ms();
-        if (c + 3 < nchunks) lines_stage0(*lease[(c + 3) % kDepth]->s, chunks[c + 3], utf8);
-        const double h1 = host_ms();
-        if (c + 1 < nchunks) lines_stage1(*p, *lease[(c + 1) % kDepth]->s, chunks[c + 1], no_norm == 0, wsconst_types, tags);
-        const double h2 = host_ms();
-        Scratch& s = *lease[c % kDepth]->s;
-        cuda_check(cudaEventSynchronize(chunks[c].done), "sync(tokenize)");
-        if (trace)
-            fprintf(stderr, "[vpt lines host] iteration %zu: begins %.3f  copy-in+split issued %.3f  kernels issued %.3f  "
-                            "chunk done seen %.3f ms\n", c, h0, h1, h2, host_ms());
-        const uint64_t nb = s.h_totals[3];
-        if (total + nb > out_capacity || (nb && !out)) overflow = true;
-        if (!overflow && nb) {
-            cuda_check(cudaMemcpyAsync(out + total, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
-            cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
-        }
-        if (pipeline_trace()) chunks[c].tr.mark(3, s.stream_out);
-        total += nb;
-        lines += chunks[c].n_lines;
-    }
-    for (int i = 0; i < kDepth; ++i)
-        if (lease[i]) {
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(tokenize)");
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
-        }
-    if (pipeline_trace())
-        for (size_t c = 0; c < nchunks; ++c) chunks[c].tr.print("lines", c, chunks[c].nbytes, chunks[0].tr);
-    if (out_len) *out_len = total;
-    if (n_lines_out) *n_lines_out = lines;
-    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: out_capacity: too small for the tokenized text");
-    return kOk;
-    VPT_API_END
-}
-}  // namespace
-
-int vpt_tokenize_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
-                       uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
-    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, false, out, out_capacity, out_len, n_lines_out);
-}
-
-int vpt_tokenize_lines_tags(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
-                            uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
-    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out);
-}
-
-namespace {
 
 // stage 1 of an evaluate chunk: line offsets, the gold parse, count + score + post-filters (+ tags) on the raw
 // sentences, the metrics; the chunk's totals and error key to pinned host memory, the per-line counts (if wanted) to
 // `line_counts` from row `line_lo`
-void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normalize, uint32_t wsconst, bool tags,
-                 int tag_mode, uint32_t* line_counts, uint64_t line_lo) {
+void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job, uint32_t* line_counts,
+                 uint64_t line_lo) {
     cudaStream_t st = s.stream;
-    cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
-    const size_t n = size_t(s.h_totals[2]);
-    ch.n_lines = n;
-    if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
+    const size_t n = split_lines(s, ch);
     if (!s.h_eval) cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s.h_eval), 8 * (kEvalTotals + 1)), "cudaMallocHost");
     if (n == 0) {
         for (int i = 0; i < kEvalTotals; ++i) s.h_eval[i] = 0;
@@ -1298,9 +1234,7 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normali
     }
     const size_t ng = (n + kGroup - 1) / kGroup;
     const size_t nb = ch.nbytes;  // bounds the surface bytes and characters of the chunk
-    Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
-    Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
+    const int tag_mode = job.tag_mode;
     Scratch::ensure(s.d_gtext, s.gtext_cap, nb + 64);
     Scratch::ensure(s.d_goff, s.goff_cap, 8 * (n + 1));
     Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
@@ -1309,12 +1243,6 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normali
     Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
     if (tag_mode == kTagsCompare) Scratch::ensure(s.d_gtag, s.gtag_cap, 4 * nb + 4);
     if (line_counts) Scratch::ensure(s.d_lc, s.lc_cap, 28 * n + 4);
-    ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
-    ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
-    // the kernels overwrite d_lc, which the previous chunk of this scratch may still be copying out
-    cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
-    if (pipeline_trace()) ch.tr.mark(1, st);
-    cuda_check(launch_split_write(ch.sp, st), "launch(split)");
     EvalArgs e;
     e.text = ch.sp.text;
     e.offsets = ch.sp.offsets;
@@ -1337,7 +1265,7 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, bool normali
     a.text = e.surface;
     a.offsets = e.surf_offsets;
     a.n_sent = n;
-    const TokArgs t = predict_lines(p, s, ch, a, nb, normalize, wsconst, tags);
+    const TokArgs t = predict_lines(p, s, ch, a, nb, job);
     e.status = t.status;
     e.n_chars = t.n_chars;
     e.boundaries = t.boundaries;
@@ -1377,154 +1305,273 @@ const char* gold_error_text(uint32_t kind) {
     }
 }
 
+// ---- the line ring: the chunk pipeline of vpt_tokenize_lines*, vpt_evaluate_lines and the line stream ----------------
+//
+// Every chunk of complete lines goes through lines_stage0 (copy-in, newline count), then lines_stage1 or eval_stage1
+// (split, scoring, post-filters, tags, output or metrics), then its owner's copy-out.  Up to kRingDepth chunks are in
+// flight, chunk c in slot c % kRingDepth on the slot's own ScratchLease, so the copy-in, kernels and copy-out of
+// neighbouring chunks overlap: the two newest chunks are copied in and counted ahead of their kernels, and the next
+// chunk's kernels are queued before the host waits for the oldest.  Chunks retire in order.  The ring knows neither where
+// a chunk's bytes come from nor where tokenised bytes go: the whole-buffer calls submit cuts of the caller's buffer and
+// copy into the caller's output, the stream submits its pinned staging buffers and hands its output to `write`.
+
+constexpr size_t kRingDepth = 4;
+
+struct LineRing {
+    struct Slot {
+        std::unique_ptr<ScratchLease> lease;
+        LineChunk ch;
+        bool stage1 = false;  // lines_stage1 / eval_stage1 issued
+        size_t index = 0;     // chunk number
+    };
+    struct Traced {  // trace events of a chunk whose slot was reused before they were printed
+        size_t index;
+        uint64_t nbytes;
+        TraceEvents tr;
+    };
+    const vpt_predictor& p;
+    const LineJob job;
+    const char* const label;  // of the trace lines
+    const bool trace;
+    Slot slots[kRingDepth];
+    size_t n_chunks = 0, n_retired = 0;  // chunks [n_retired, n_chunks) are in flight
+    uint64_t lines = 0, tot[kEvalTotals] = {};  // of the retired chunks
+    // per-line counts of the whole-buffer evaluate call (none: nullptr); a chunk's rows go out only while the buffer has
+    // room for all of them
+    uint32_t* line_counts = nullptr;
+    uint64_t line_capacity = 0, lines_issued = 0;
+    bool counts_overflow = false;
+    TraceEvents t0;  // trace origin: before the first chunk's copy-in
+    std::vector<Traced> traced;
+
+    LineRing(const vpt_predictor& pr, const LineJob& j, const char* what)
+        : p(pr), job(j), label(what), trace(pipeline_trace()) {}
+
+    ~LineRing() {
+        // last slot first, so that slot 0's scratch is the next one leased: a later ring's slot 0 takes it again
+        for (size_t i = kRingDepth; i-- > 0;) {
+            Slot& sl = slots[i];
+            sl.lease.reset();  // synchronises the lease's streams and hands its scratch back to the predictor
+            if (sl.ch.split) cudaEventDestroy(sl.ch.split);
+            if (sl.ch.done) cudaEventDestroy(sl.ch.done);
+            sl.ch.tr.destroy();
+        }
+        for (Traced& t : traced) t.tr.destroy();
+        t0.destroy();
+    }
+
+    Slot& slot(size_t chunk) { return slots[chunk % kRingDepth]; }
+    bool full() const { return n_chunks - n_retired == kRingDepth; }
+
+    // queues a chunk of `n` bytes of complete lines at `bytes`, which stay untouched until it retires; the ring must not
+    // be full
+    void submit(const uint8_t* bytes, size_t n) {
+        Slot& sl = slot(n_chunks);  // chunks retire in order: this slot is free
+        if (!sl.lease) sl.lease.reset(new ScratchLease(p));
+        if (sl.ch.tr.ev[0]) {
+            // the slot's last chunk is not printed yet, and its copy-out may still be running
+            traced.push_back({sl.index, sl.ch.nbytes, sl.ch.tr});
+            sl.ch.tr = TraceEvents();
+        }
+        sl.ch.nbytes = n;
+        sl.ch.n_lines = 0;
+        sl.stage1 = false;
+        sl.index = n_chunks++;
+        Scratch& s = *sl.lease->s;
+        if (trace && sl.index == 0) t0.mark(0, s.stream);
+        lines_stage0(s, sl.ch, bytes);
+        for (size_t c = n_retired; c + 2 < n_chunks; ++c)
+            if (!slot(c).stage1) issue(slot(c));
+    }
+
+    void issue(Slot& sl) {
+        Scratch& s = *sl.lease->s;
+        if (job.kind == VPT_STREAM_TOKENIZE) {
+            lines_stage1(p, s, sl.ch, job);
+        } else {
+            uint32_t* counts = nullptr;
+            if (line_counts) {
+                // the chunk's line count is known once its split pass is done
+                cuda_check(cudaEventSynchronize(sl.ch.split), "sync(split)");
+                if (lines_issued + s.h_totals[2] <= line_capacity) counts = line_counts;
+                else counts_overflow = true;
+            }
+            eval_stage1(p, s, sl.ch, job, counts, lines_issued);
+            lines_issued += sl.ch.n_lines;
+        }
+        sl.stage1 = true;
+    }
+
+    // Waits for the oldest chunk and takes it out of the ring: its lines are counted and, for evaluate, its error key is
+    // checked and its totals are added.  Chunks retire in line order, so the first error met is the lowest bad line's.
+    // The owner copies the chunk's output out of the returned slot before the next submit reuses it.
+    Slot& retire() {
+        // the next chunk's kernels are queued before the host waits for the oldest
+        for (size_t c = n_retired; c < std::min(n_retired + 2, n_chunks); ++c)
+            if (!slot(c).stage1) issue(slot(c));
+        Slot& sl = slot(n_retired);
+        Scratch& s = *sl.lease->s;
+        cuda_check(cudaEventSynchronize(sl.ch.done), "sync(lines)");
+        if (job.kind == VPT_STREAM_EVALUATE) {
+            const uint64_t key = s.h_eval[kEvalTotals];
+            if (key != kGoldNoError) {
+                const uint64_t line = lines + (key >> 34);
+                const uint32_t kind = uint32_t(key & 7u);
+                if (kind == kGoldUtf8)
+                    throw Error(kIoError, "stream did not contain valid UTF-8 (line " + std::to_string(line) + ")");
+                throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind) +
+                                                  " (line " + std::to_string(line) + ")");
+            }
+            for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
+        }
+        lines += sl.ch.n_lines;
+        ++n_retired;
+        return sl;
+    }
+
+    void drain(const std::function<void(Slot&)>& deliver) {
+        while (n_retired < n_chunks) deliver(retire());
+    }
+
+    // A whole buffer through the ring, in the chunks of line_chunks; `deliver` takes every retired slot.  The final
+    // synchronisation is checked: a failed copy-out is an error of the call, not left to the leases' release.
+    void run(const uint8_t* utf8, size_t n_bytes, const std::function<void(Slot&)>& deliver) {
+        size_t lo = 0;
+        for (const size_t hi : line_chunks(utf8, n_bytes)) {
+            if (full()) deliver(retire());
+            submit(utf8 + lo, hi - lo);
+            lo = hi;
+        }
+        drain(deliver);
+        for (Slot& sl : slots)
+            if (sl.lease) {
+                cuda_check(cudaStreamSynchronize(sl.lease->s->stream), "sync(lines)");
+                cuda_check(cudaStreamSynchronize(sl.lease->s->stream_out), "sync(copy-out)");
+            }
+        if (!trace) return;
+        for (const Traced& t : traced) t.tr.print(label, t.index, t.nbytes, t0);
+        for (size_t k = 0; k < kRingDepth; ++k) {
+            Slot& sl = slot(n_chunks + k);  // oldest first
+            if (sl.ch.tr.ev[0]) print(sl);
+        }
+    }
+
+    // prints the trace line of a retired chunk whose events are complete, and frees them
+    void print(Slot& sl) {
+        sl.ch.tr.print(label, sl.index, sl.ch.nbytes, t0);
+        sl.ch.tr.destroy();
+    }
+
+    vpt_eval_counts counts() const {
+        vpt_eval_counts c = vpt_eval_counts();
+        c.n_lines = lines;
+        c.tp = tot[0];
+        c.tn = tot[1];
+        c.fp = tot[2];
+        c.fn = tot[3];
+        c.n_sys = tot[4];
+        c.n_ref = tot[5];
+        c.n_cor = tot[6];
+        c.n_sentences = tot[7];
+        return c;
+    }
+};
+
+int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
+                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    VPT_API_BEGIN
+    const LineJob job = line_job(p, VPT_STREAM_TOKENIZE, no_norm, wsconst_types, tags);
+    if (out_len) *out_len = 0;
+    if (n_lines_out) *n_lines_out = 0;
+    if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
+    if (n_bytes == 0) return kOk;
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    LineRing ring(*p, job, "lines");
+    uint64_t total = 0;  // counts on past an overflow: *out_len is the size needed
+    bool overflow = false;
+    ring.run(utf8, n_bytes, [&](LineRing::Slot& sl) {
+        // the copy-out overlaps the next chunks' copy-in and kernels; the ring's final synchronisation waits for it
+        Scratch& s = *sl.lease->s;
+        const uint64_t nb = s.h_totals[3];
+        if (total + nb > out_capacity || (nb && !out)) overflow = true;
+        if (!overflow && nb) {
+            cuda_check(cudaMemcpyAsync(out + total, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
+            cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
+        }
+        if (ring.trace) sl.ch.tr.mark(3, s.stream_out);
+        total += nb;
+    });
+    if (out_len) *out_len = total;
+    if (n_lines_out) *n_lines_out = ring.lines;
+    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: out_capacity: too small for the tokenized text");
+    return kOk;
+    VPT_API_END
+}
+
 }  // namespace
+
+int vpt_tokenize_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
+                       uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, false, out, out_capacity, out_len, n_lines_out);
+}
+
+int vpt_tokenize_lines_tags(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
+                            uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out);
+}
 
 int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
                        int predict_tags, vpt_eval_counts* out, uint32_t* line_counts, uint64_t line_capacity) {
     VPT_API_BEGIN
-    const bool tags = check_lines_flags(p, wsconst_types, predict_tags != 0);
+    const LineJob job = line_job(p, VPT_STREAM_EVALUATE, no_norm, wsconst_types, predict_tags != 0);
     if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
     *out = vpt_eval_counts();
     if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     if (n_bytes == 0) return kOk;
-    // main.rs:110-120 with predictor.rs:553: the system keeps the gold tags (--no-norm) or has none, unless tags are
-    // predicted with a model that has tag slots
-    const int tag_mode = tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-
-    std::vector<LineChunk> chunks = line_chunks(utf8, n_bytes);
-    const size_t nchunks = chunks.size();
-    constexpr int kDepth = 4;
-    std::unique_ptr<ScratchLease> lease[kDepth];
-    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
-    struct EventGuard {
-        std::vector<LineChunk>& c;
-        ~EventGuard() {
-            for (auto& x : c) {
-                if (x.split) cudaEventDestroy(x.split);
-                if (x.done) cudaEventDestroy(x.done);
-                x.tr.destroy();
-            }
-        }
-    } guard{chunks};
-
-    // as tokenize_lines_impl: chunks c+2, c+3 are copied in and split while chunk c+1 is parsed, scored and evaluated
-    uint64_t lines_issued = 0, lines = 0, tot[kEvalTotals] = {};
-    bool overflow = false;
-    auto stage1 = [&](size_t c) {
-        Scratch& s = *lease[c % kDepth]->s;
-        // per-line counts go out only while the buffer has room for the chunk (its line count is known in the stage)
-        cuda_check(cudaEventSynchronize(chunks[c].split), "sync(split)");
-        const uint64_t n = s.h_totals[2];
-        const bool fits = line_counts && lines_issued + n <= line_capacity;
-        if (line_counts && !fits) overflow = true;
-        eval_stage1(*p, s, chunks[c], no_norm == 0, wsconst_types, tags, tag_mode, fits ? line_counts : nullptr, lines_issued);
-        lines_issued += n;
-    };
-    for (size_t c = 0; c < std::min<size_t>(3, nchunks); ++c) lines_stage0(*lease[c % kDepth]->s, chunks[c], utf8);
-    stage1(0);
-    for (size_t c = 0; c < nchunks; ++c) {
-        if (c + 3 < nchunks) lines_stage0(*lease[(c + 3) % kDepth]->s, chunks[c + 3], utf8);
-        if (c + 1 < nchunks) stage1(c + 1);
-        Scratch& s = *lease[c % kDepth]->s;
-        cuda_check(cudaEventSynchronize(chunks[c].done), "sync(evaluate)");
-        const uint64_t key = s.h_eval[kEvalTotals];
-        if (key != kGoldNoError) {
-            // chunks are checked in line order: the first chunk with an error holds the lowest bad line
-            const uint64_t line = lines + (key >> 34);
-            const uint32_t kind = uint32_t(key & 7u);
-            if (kind == kGoldUtf8)
-                throw Error(kIoError, "stream did not contain valid UTF-8 (line " + std::to_string(line) + ")");
-            throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind) +
-                                              " (line " + std::to_string(line) + ")");
-        }
-        for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
-        lines += chunks[c].n_lines;
-    }
-    for (int i = 0; i < kDepth; ++i)
-        if (lease[i]) {
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(evaluate)");
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
-        }
-    if (pipeline_trace())
-        for (size_t c = 0; c < nchunks; ++c) chunks[c].tr.print("evaluate", c, chunks[c].nbytes, chunks[0].tr);
-    out->n_lines = lines;
-    out->tp = tot[0];
-    out->tn = tot[1];
-    out->fp = tot[2];
-    out->fn = tot[3];
-    out->n_sys = tot[4];
-    out->n_ref = tot[5];
-    out->n_cor = tot[6];
-    out->n_sentences = tot[7];
-    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: line_capacity: too small for the lines");
+    LineRing ring(*p, job, "evaluate");
+    ring.line_counts = line_counts;
+    ring.line_capacity = line_capacity;
+    ring.run(utf8, n_bytes, [](LineRing::Slot&) {});
+    *out = ring.counts();
+    if (ring.counts_overflow) throw Error(kInvalidArgument, "InvalidArgumentError: line_capacity: too small for the lines");
     return kOk;
     VPT_API_END
 }
 
 // ---- line stream: the loops of vpt_tokenize_lines* and vpt_evaluate_lines, fed in pieces ----------------------------
 //
-// The stream cuts its input into chunks of complete lines in pinned staging buffers (line_feed.hpp) and drives every
-// chunk through the per-chunk stages of the whole-buffer drivers, in their order: lines_stage0 (copy-in, newline count),
-// lines_stage1 or eval_stage1 (split, scoring, output or metrics), then the copy-out.  Up to kStreamDepth chunks are in
-// flight, each on its own ScratchLease, so the copy-in, kernels and copy-out of neighbouring chunks overlap.  The
-// whole-buffer drivers keep their own loops: they read the caller's buffer in place, without a staging copy.
-// Invariants: a slot's pinned input buffer is not refilled before its chunk retires, which is after the chunk's `done`
-// event (recorded after its H2D, on the same stream) has completed; the pinned output buffer is not reused before the
-// `write` call that consumed it has returned (chunks retire one at a time, on the caller's thread).
-
-namespace {
-constexpr size_t kStreamDepth = 4;
-}  // namespace
+// The stream cuts its input into chunks of complete lines in pinned staging buffers (line_feed.hpp) and submits them to
+// a LineRing.  Invariants: a slot's pinned input buffer is not refilled before its chunk retires, which is after the
+// chunk's `done` event (recorded after its H2D, on the same stream) has completed; the pinned output buffer is not reused
+// before the `write` call that consumed it has returned (chunks retire one at a time, on the caller's thread).
 
 struct vpt_line_stream {
-    struct Slot {
-        std::unique_ptr<ScratchLease> lease;
-        LineChunk ch;
-        FeedBuf in;           // the chunk's pinned input
-        bool stage1 = false;  // lines_stage1 / eval_stage1 issued
-        size_t index = 0;     // chunk number (trace)
-    };
     const vpt_predictor* p;
-    const int kind;
-    const bool normalize, tags;
-    const uint32_t wsconst;
-    const int tag_mode;
     const vpt_stream_write_fn write;
     void* const ctx;
-    const bool trace;
     const size_t big;               // nominal chunk size (VPT_CHUNK_BYTES)
-    Slot slots[kStreamDepth];
-    std::deque<size_t> fifo;        // slots in flight, oldest first
-    size_t n_chunks = 0;
+    std::unique_ptr<LineRing> ring;
+    FeedBuf in[kRingDepth];         // the pinned input of the chunk in each slot of the ring
     std::vector<FeedBuf> spare;     // input buffers of retired chunks
     // every pinned buffer of the stream (pointer, bytes); the destructor hands them to the predictor's pool
     std::vector<std::pair<uint8_t*, size_t>> pinned;
     FeedBuf out;                    // pinned output staging (tokenize), sized by the largest chunk output seen
     LineFeed<vpt_line_stream> feed;
-    uint64_t lines = 0, tot[kEvalTotals] = {};
-    TraceEvents t0;                 // trace origin: before the first chunk's copy-in
     int status = kOk;               // an earlier error: every later call returns it again with `message`
     std::string message;
     bool finished = false;
 
-    vpt_line_stream(const vpt_predictor* pr, int k, bool norm, uint32_t ws, bool tg, int tm, vpt_stream_write_fn w, void* c)
-        : p(pr), kind(k), normalize(norm), tags(tg), wsconst(ws), tag_mode(tm), write(w), ctx(c), trace(pipeline_trace()),
-          big(chunk_bytes()), feed(*this, big, kMaxLineChunk) {}
+    vpt_line_stream(const vpt_predictor* pr, const LineJob& job, vpt_stream_write_fn w, void* c)
+        : p(pr), write(w), ctx(c), big(chunk_bytes()), ring(new LineRing(*pr, job, "stream")), feed(*this, big, kMaxLineChunk) {}
 
     ~vpt_line_stream() {
-        for (Slot& sl : slots) {
-            sl.lease.reset();  // synchronises the lease's streams and hands its scratch back to the predictor
-            if (sl.ch.split) cudaEventDestroy(sl.ch.split);
-            if (sl.ch.done) cudaEventDestroy(sl.ch.done);
-            sl.ch.tr.destroy();
-        }
-        t0.destroy();
+        ring.reset();  // its leases synchronise their streams: no copy reads the pinned buffers any more
         // pinning memory costs more than a short stream's work: the buffers of chunk size are kept for later streams
-        // (at most kStreamDepth + 2 per concurrent stream), the others are freed
+        // (at most kRingDepth + 2 per concurrent stream), the others are freed
         std::lock_guard<std::mutex> g(p->mu);
         for (const auto& b : pinned) {
-            if (b.second <= 2 * big + big / 2 && p->pinned_pool.size() < 4 * (kStreamDepth + 2)) p->pinned_pool.push_back(b);
+            if (b.second <= 2 * big + big / 2 && p->pinned_pool.size() < 4 * (kRingDepth + 2)) p->pinned_pool.push_back(b);
             else cudaFreeHost(b.first);
         }
     }
@@ -1556,7 +1603,7 @@ struct vpt_line_stream {
 
     // -- LineFeed's host: buffers and chunks
     FeedBuf fresh(size_t min_cap) {
-        if (spare.empty() && fifo.size() == kStreamDepth) retire();
+        if (spare.empty() && ring->full()) deliver(ring->retire());
         FeedBuf b;
         if (!spare.empty()) { b = spare.back(); spare.pop_back(); }
         b.size = 0;
@@ -1579,43 +1626,18 @@ struct vpt_line_stream {
     }
     [[noreturn]] void too_long() { throw Error(kInvalidArgument, "InvalidArgumentError: utf8: a line is longer than 1 GiB"); }
     void emit(FeedBuf& b) {
-        if (fifo.size() == kStreamDepth) retire();
-        const size_t i = n_chunks % kStreamDepth;  // chunks retire in order: this slot is free
-        Slot& sl = slots[i];
-        sl.in = b;
+        if (ring->full()) deliver(ring->retire());
+        FeedBuf& slot_in = in[ring->n_chunks % kRingDepth];  // the slot the chunk goes to
+        slot_in = b;
         b = FeedBuf();
-        if (!sl.lease) sl.lease.reset(new ScratchLease(*p));
-        sl.ch.byte_lo = 0;
-        sl.ch.nbytes = sl.in.size;
-        sl.ch.n_lines = 0;
-        sl.stage1 = false;
-        sl.index = n_chunks++;
-        Scratch& s = *sl.lease->s;
-        if (trace && sl.index == 0) t0.mark(0, s.stream);
-        fifo.push_back(i);
-        lines_stage0(s, sl.ch, sl.in.data);
-        // as in the whole-buffer drivers, the two newest chunks are copied in and counted ahead of their kernels
-        for (size_t k = 0; k + 2 < fifo.size(); ++k)
-            if (!slots[fifo[k]].stage1) issue(slots[fifo[k]]);
+        ring->submit(slot_in.data, slot_in.size);
     }
 
-    void issue(Slot& sl) {
-        Scratch& s = *sl.lease->s;
-        if (kind == VPT_STREAM_TOKENIZE) lines_stage1(*p, s, sl.ch, normalize, wsconst, tags);
-        else eval_stage1(*p, s, sl.ch, normalize, wsconst, tags, tag_mode, nullptr, 0);
-        sl.stage1 = true;
-    }
-
-    // waits for the oldest chunk and delivers it: its output to `write` (tokenize) or its totals (evaluate)
-    void retire() {
-        // the next chunk's kernels are queued before the host waits for the oldest
-        for (size_t k = 0; k < std::min<size_t>(2, fifo.size()); ++k)
-            if (!slots[fifo[k]].stage1) issue(slots[fifo[k]]);
-        Slot& sl = slots[fifo.front()];
-        Scratch& s = *sl.lease->s;
-        cuda_check(cudaEventSynchronize(sl.ch.done), "sync(stream)");
+    // delivers a retired chunk: its output to `write` (tokenize; the ring keeps the evaluate totals)
+    void deliver(LineRing::Slot& sl) {
         uint64_t nb = 0;
-        if (kind == VPT_STREAM_TOKENIZE) {
+        if (ring->job.kind == VPT_STREAM_TOKENIZE) {
+            Scratch& s = *sl.lease->s;
             nb = s.h_totals[3];
             if (nb > out.cap) {
                 release(out.data);
@@ -1623,32 +1645,18 @@ struct vpt_line_stream {
                 out.data = alloc(out.cap);
             }
             if (nb) cuda_check(cudaMemcpyAsync(out.data, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
-            if (trace) sl.ch.tr.mark(3, s.stream_out);
+            if (ring->trace) sl.ch.tr.mark(3, s.stream_out);
             cuda_check(cudaStreamSynchronize(s.stream_out), "sync(copy-out)");
-        } else {
-            // chunks retire in line order: the first chunk with an error holds the lowest bad line (as vpt_evaluate_lines
-            // reports it)
-            const uint64_t key = s.h_eval[kEvalTotals];
-            if (key != kGoldNoError) {
-                const uint64_t line = lines + (key >> 34);
-                const uint32_t kind_ = uint32_t(key & 7u);
-                if (kind_ == kGoldUtf8)
-                    throw Error(kIoError, "stream did not contain valid UTF-8 (line " + std::to_string(line) + ")");
-                throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind_) +
-                                                  " (line " + std::to_string(line) + ")");
-            }
-            for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
         }
-        if (trace) sl.ch.tr.print("stream", sl.index, sl.ch.nbytes, t0);
-        lines += sl.ch.n_lines;
-        fifo.pop_front();
-        spare.push_back(sl.in);
-        sl.in = FeedBuf();
+        if (ring->trace) ring->print(sl);
+        FeedBuf& slot_in = in[sl.index % kRingDepth];
+        spare.push_back(slot_in);
+        slot_in = FeedBuf();
         if (nb && write(ctx, out.data, size_t(nb)) != 0) throw Error(kIoError, "write callback failed");
     }
 
     void drain() {
-        while (!fifo.empty()) retire();
+        ring->drain([this](LineRing::Slot& sl) { deliver(sl); });
     }
 };
 
@@ -1686,12 +1694,10 @@ int vpt_line_stream_new(const vpt_predictor* p, int kind, int no_norm, uint32_t 
     *out = nullptr;
     if (kind != VPT_STREAM_TOKENIZE && kind != VPT_STREAM_EVALUATE)
         throw Error(kInvalidArgument, "InvalidArgumentError: kind: VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE");
-    const bool tags = check_lines_flags(p, wsconst_types, predict_tags != 0);
+    const LineJob job = line_job(p, kind, no_norm, wsconst_types, predict_tags != 0);
     if (kind == VPT_STREAM_TOKENIZE && !write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
-    // as vpt_evaluate_lines: the system keeps the gold tags (no_norm) or has none, unless tags are predicted
-    const int tag_mode = tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-    *out = new vpt_line_stream(p, kind, no_norm == 0, wsconst_types, tags, tag_mode, write, ctx);
+    *out = new vpt_line_stream(p, job, write, ctx);
     return kOk;
     VPT_API_END
 }
@@ -1717,18 +1723,8 @@ int vpt_line_stream_finish(vpt_line_stream* st, uint64_t* n_lines, vpt_eval_coun
         st->feed.finish();
         st->drain();
         st->finished = true;
-        if (n_lines) *n_lines = st->lines;
-        if (counts && st->kind == VPT_STREAM_EVALUATE) {
-            counts->n_lines = st->lines;
-            counts->tp = st->tot[0];
-            counts->tn = st->tot[1];
-            counts->fp = st->tot[2];
-            counts->fn = st->tot[3];
-            counts->n_sys = st->tot[4];
-            counts->n_ref = st->tot[5];
-            counts->n_cor = st->tot[6];
-            counts->n_sentences = st->tot[7];
-        }
+        if (n_lines) *n_lines = st->ring->lines;
+        if (counts && st->ring->job.kind == VPT_STREAM_EVALUATE) *counts = st->ring->counts();
     });
 }
 
