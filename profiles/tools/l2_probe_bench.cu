@@ -5,7 +5,9 @@
 //   mkdir -p build && nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/l2_probe_bench profiles/tools/l2_probe_bench.cu
 //   build/l2_probe_bench > build/l2_probe_bench.jsonl
 // Output: one JSON object per line {"test": ..., "table_mb": ..., "ilp": ..., "gprobes_s": ..., "gbs": ...}.
-// The numbers give the peak of the scoring kernel's second roofline (bench.py: roofline_l1_lines).
+// The numbers give the peak of the scoring kernel's second roofline (bench.py: roofline_l1_lines).  "record_load" is
+// the test with load_record's own instructions and k_fused's geometry; the older "record32" kernels and the 32- and
+// 128-byte "variant" kernels read only some words of a record, and ptxas narrows those loads to 32-bit ones.
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -96,6 +98,110 @@ __global__ void __launch_bounds__(1024) k_probe_var(const void* table, uint32_t 
         idx = mix(idx + 0x632BE5ABu);
     }
     if (acc == 0x12345678u) *sink = acc;
+}
+
+// ---- record load forms (load_record in vaporetto_b200/csrc/kernels_common.cuh), at k_fused's geometry ---------------
+// na2     two v4 loads, L1::no_allocate + evict-last L2 hint (the kernel's load): two L2 sector requests per record
+// l1a2    the same two loads allocating in L1 (the second may hit the line the first brought in)
+// l1a2ef  as l1a2 with L1::evict_first
+// pair    lanes 2k / 2k+1 read the two halves of one record in one instruction (one sector request per record), four
+//         shuffles give each lane the half its partner read
+// one16   one v4 load per record: the one-request lower bound (not a record format)
+enum Mode { kNa2, kL1a2, kL1a2ef, kPair, kOne16 };
+
+__device__ __forceinline__ uint64_t pol_last() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t pol_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+
+template <int kMode>
+__device__ __forceinline__ void ld16(const char* p, uint64_t pol, uint32_t (&v)[4]) {
+    if (kMode == kL1a2)
+        asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p), "l"(pol));
+    else if (kMode == kL1a2ef)
+        asm volatile("ld.global.nc.L1::evict_first.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p), "l"(pol));
+    else
+        asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p), "l"(pol));
+}
+
+// the record of `slot`, loaded in form kMode (called by the whole warp for kPair)
+template <int kMode>
+__device__ __forceinline__ Rec32 load_mode(const char* table, uint32_t slot, uint32_t lane, uint64_t pol) {
+    Rec32 r;
+    uint32_t a[4], b[4];
+    if (kMode == kPair) {
+        const uint32_t odd = lane & 1u;
+        const uint32_t se = __shfl_sync(0xFFFFFFFFu, slot, lane & ~1u), so = __shfl_sync(0xFFFFFFFFu, slot, lane | 1u);
+        // both lanes of a pair read the even lane's record, then the odd lane's; each keeps half 0 of its own record
+        ld16<kNa2>(table + (size_t(se) << 5) + 16u * odd, pol, a);
+        ld16<kNa2>(table + (size_t(so) << 5) + 16u * (odd ^ 1u), pol, b);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t keep = odd ? b[j] : a[j], send = odd ? a[j] : b[j];
+            r.v[j] = keep;
+            r.v[4 + j] = __shfl_xor_sync(0xFFFFFFFFu, send, 1);
+        }
+    } else if (kMode == kOne16) {
+        ld16<kNa2>(table + (size_t(slot) << 5), pol, a);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { r.v[j] = a[j]; r.v[4 + j] = a[j] >> 1; }
+    } else {
+        ld16<kMode>(table + (size_t(slot) << 5), pol, a);
+        ld16<kMode>(table + (size_t(slot) << 5) + 16, pol, b);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { r.v[j] = a[j]; r.v[4 + j] = b[j]; }
+    }
+    return r;
+}
+
+// One 1024-thread CTA per SM with k_fused's shared-memory footprint (so L1 is as small as the kernel's).  With kStream,
+// every fourth warp streams instead of probing: 16 B per lane and iteration read with an evict-first hint (the text's
+// bulk copy) and 16 B written with a streaming store (the outputs), through buffers larger than L2 -- about 5 B per
+// probe, k_fused's ratio of streamed bytes to record probes.  Without it those warps idle, so the probe count is the same.
+template <int kMode, bool kStream>
+__global__ void __launch_bounds__(1024, 1) k_probe_mode(const char* table, uint32_t nslots, int iters, const uint4* sin,
+                                                         uint4* sout, size_t nvec, uint32_t* sink) {
+    extern __shared__ uint8_t s_pad[];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t acc = 0;
+    if ((warp & 3) == 3) {
+        if (!kStream) return;
+        const uint64_t pf = pol_first();
+        const size_t sw = size_t(blockIdx.x) * 8 + (warp >> 2), nsw = size_t(gridDim.x) * 8;
+        for (int i = 0; i < iters; ++i) {
+            const size_t k = ((size_t(i) * nsw + sw) * 32 + lane) % nvec;
+            uint32_t v[4];
+            asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(sin + k), "l"(pf));
+            __stcs(sout + k, make_uint4(v[0] + i, v[1], v[2], v[3]));
+        }
+        return;
+    }
+    const uint64_t pol = pol_last();
+    uint32_t idx[2] = {mix(tid * 2 + 1), mix(tid * 2 + 2)};
+    for (int i = 0; i < iters; ++i) {
+        Rec32 r[2];
+#pragma unroll
+        for (int j = 0; j < 2; ++j) r[j] = load_mode<kMode>(table, uint32_t((uint64_t(idx[j]) * nslots) >> 32), lane, pol);
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            // (every word: ptxas narrows a vector load whose other words are unused)
+#pragma unroll
+            for (int w = 0; w < 8; ++w) acc += r[j].v[w] << w;
+            idx[j] = mix(idx[j] + 0x632BE5ABu);
+        }
+    }
+    if (acc == 0x12345678u) *sink = acc + s_pad[0];
 }
 
 // random byte reads from a 37 KB shared-memory table (the perfect-hash seeds): LDS.U8 with random bank pattern
@@ -206,6 +312,45 @@ int main() {
                    x.name, mb, x.ms, probes / x.ms / 1e6, probes * 32.0 / x.ms / 1e6, probes / x.ms / 1e3 / n_sm / clk_khz);
         }
         fflush(stdout);
+    }
+    {   // the record load forms at k_fused's geometry, alone and beside streaming traffic
+        const size_t stream_bytes = size_t(64) << 20;  // each of the two streamed buffers: larger than the 50 MB L2
+        uint4 *sin, *sout;
+        CK(cudaMalloc(&sin, stream_bytes));
+        CK(cudaMalloc(&sout, stream_bytes));
+        CK(cudaMemset(sin, 0x11, stream_bytes));
+        const size_t nvec = stream_bytes / 16;
+        const int smem = 220 * 1024;  // k_fused's 217-227 KB: the L1 that is left is the kernel's
+        const int iters = 256;
+        struct M { const char* name; void (*k0)(const char*, uint32_t, int, const uint4*, uint4*, size_t, uint32_t*);
+                   void (*k1)(const char*, uint32_t, int, const uint4*, uint4*, size_t, uint32_t*); } modes[] = {
+            {"na2", k_probe_mode<kNa2, false>, k_probe_mode<kNa2, true>},
+            {"l1a2", k_probe_mode<kL1a2, false>, k_probe_mode<kL1a2, true>},
+            {"l1a2ef", k_probe_mode<kL1a2ef, false>, k_probe_mode<kL1a2ef, true>},
+            {"pair", k_probe_mode<kPair, false>, k_probe_mode<kPair, true>},
+            {"one16", k_probe_mode<kOne16, false>, k_probe_mode<kOne16, true>}};
+        for (const M& x : modes)
+            for (auto k : {x.k0, x.k1}) CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        const double mode_mb[] = {8, 17.1, 23};
+        // probing warps: three of every four, two independent records in flight per lane
+        const double probes = double(n_sm) * 1024 * 3 / 4 * iters * 2;
+        for (double mb : mode_mb) {
+            const uint32_t nslots = uint32_t(mb * 1048576.0 / 32.0);
+            for (int stream = 0; stream < 2; ++stream) {
+                for (const M& x : modes) {
+                    auto k = stream ? x.k1 : x.k0;
+                    const float ms = time_ms([&] { k<<<n_sm, 1024, smem>>>(static_cast<const char*>(table), nslots, iters, sin, sout, nvec, sink); }, 10);
+                    printf("{\"test\": \"record_load\", \"mode\": \"%s\", \"table_mb\": %.1f, \"streaming\": %s, \"ms\": %.4f, "
+                           "\"gprobes_s\": %.2f, \"stream_gbs\": %.1f}\n",
+                           x.name, mb, stream ? "true" : "false", ms, probes / ms / 1e6,
+                           stream ? double(n_sm) * 8 * iters * 1024.0 / ms / 1e6 : 0.0);
+                }
+                fflush(stdout);
+            }
+        }
+        CK(cudaGetLastError());
+        CK(cudaFree(sin));
+        CK(cudaFree(sout));
     }
     {
         const int iters = 256;
