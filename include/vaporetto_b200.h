@@ -440,6 +440,50 @@ int vpt_line_stream_flush(vpt_line_stream* stream);
 int vpt_line_stream_finish(vpt_line_stream* stream, uint64_t* n_lines, vpt_eval_counts* counts /* EVALUATE only */);
 void vpt_line_stream_free(vpt_line_stream* stream);
 
+/* ---- Tag rules: vaporetto_rules' PatternMatchTagger in the tagged line path --------------------------------------------
+ *
+ * `PatternMatchTagger::new(rules)` and `filter` (vaporetto_rules/src/sentence_filters/pattern_match_tagger.rs:21-41): a
+ * table surface -> [Option<tag>] that supplies tags the model does not predict, typically for out-of-vocabulary words
+ * (proper nouns, product names) from a user dictionary.  The filter runs on the sentence that was predicted, right after
+ * fill_tags, as if the `predict` CLI's loop called it there (main.rs:130-136,157-159); the tags are then copied to the
+ * original line as usual.  For every token, every tag slot j < n_tags that is still None after tag prediction becomes
+ * rules[surface][j] when the surface is a key; a rule with fewer entries leaves the later slots None, entries beyond
+ * n_tags are ignored, and predicted tags are never overwritten.  Some("") is a tag: it writes a '/' with nothing after
+ * it and counts for the last slot written.  With n_tags == 0 (no tag models) the rules do nothing, and rejected lines
+ * (invalid UTF-8, U+0000) still print an empty line.
+ * Surface matching: unless no_norm, a token is matched by its KyteaFullwidthFilter image, because that is the sentence
+ * the filter sees.  Rule keys are not normalised: a half-width key ("ABC") matches only with no_norm; give the
+ * full-width key ("ＡＢＣ") for the default.
+ *
+ * Layout: rule i has the surface surfaces[surface_offsets[i] .. surface_offsets[i+1]) and the tag slots
+ * slot_offsets[i] .. slot_offsets[i+1]; slot k is the pair slots[2k] (offset into `tags`, or UINT32_MAX for None),
+ * slots[2k+1] (length; 0 is Some("")).  surface_offsets and slot_offsets have n_rules + 1 entries.  Everything is
+ * copied: the caller's arrays may be freed on return.  Errors (VPT_INVALID_ARGUMENT, naming the rule): NULL arrays, an
+ * offset that decreases or a tag outside `tags`, a surface or tag that is not valid UTF-8, a duplicate surface.  An
+ * empty surface, or one containing U+0000, is accepted and never matches.
+ * The rules are bound to `predictor` (its device and its n_tags: slots beyond it are dropped here) and must outlive
+ * every call and line stream that uses them; they are read-only and may be shared by concurrent calls.  Rules on a
+ * call without tag prediction, or with no rules at all, change nothing: the output is that of the call without rules. */
+typedef struct vpt_tag_rules vpt_tag_rules;
+int vpt_tag_rules_new(const vpt_predictor* predictor, uint64_t n_rules, const uint8_t* surfaces,
+                      const uint64_t* surface_offsets, const uint64_t* slot_offsets, const uint32_t* slots,
+                      const uint8_t* tags, uint64_t tags_len, vpt_tag_rules** out);
+void vpt_tag_rules_free(vpt_tag_rules* rules);
+/* The largest device output buffer, in bytes, that a chunk of a call with these rules has used (a diagnostic of the
+ * output sizing: a chunk's buffer is sized by the rule suffixes its tokens actually matched, not by the longest rule). */
+uint64_t vpt_tag_rules_max_output(const vpt_tag_rules* rules);
+
+/* vpt_tokenize_lines_tags with `rules` (nullable: NULL is vpt_tokenize_lines_tags).  Same arguments and errors; a rule's
+ * tag can be long, so `out` needs room for the matched rule tags too, and *out_len reports the size needed. */
+int vpt_tokenize_lines_tags_rules(const vpt_predictor* predictor, const vpt_tag_rules* rules, const uint8_t* utf8,
+                                  size_t n_bytes, int no_norm, uint32_t wsconst_types, uint8_t* out, size_t out_capacity,
+                                  uint64_t* out_len, uint64_t* n_lines);
+/* vpt_line_stream_new with `rules` (nullable), applied as in vpt_tokenize_lines_tags_rules on a VPT_STREAM_TOKENIZE
+ * stream with predict_tags; ignored otherwise. */
+int vpt_line_stream_new_rules(const vpt_predictor* predictor, const vpt_tag_rules* rules, int kind, int no_norm,
+                              uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
+                              vpt_line_stream** out);
+
 /* ---- Token spans: vaporetto_tantivy's token_stream for a batch of documents ---------------------------------------
  *
  * `VaporettoTokenizer::token_stream` (vaporetto_tantivy/src/lib.rs:157-229) on the device, for many documents: only text

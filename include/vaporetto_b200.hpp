@@ -105,6 +105,11 @@ struct Token {
     std::vector<std::optional<std::string>> tags() const;
 };
 
+class TagRules;
+namespace detail {
+inline const vpt_tag_rules* rules_handle(const TagRules* r);
+}
+
 /// `vaporetto::Predictor` resident on one CUDA device.
 class Predictor {
 public:
@@ -125,16 +130,17 @@ public:
     /// `vpt_tokenize_lines`): line splitting, the KyteaFullwidthFilter pre-filter (unless `no_norm`), prediction and
     /// `write_tokenized_text` + '\n' all run on the device.  Returns the output text.
     /// `predict_tags`: the CLI's --predict-tags (`vpt_tokenize_lines_tags`: fill_tags + tags in the output text).
+    /// `tag_rules`: PatternMatchTagger after fill_tags (`vpt_tokenize_lines_tags_rules`; with predict_tags only).
     std::string tokenize_lines(const std::string& text, bool no_norm = false, uint32_t wsconst_types = 0,
-                               bool predict_tags = false) const {
+                               bool predict_tags = false, const TagRules* tag_rules = nullptr) const {
         size_t n_lines = 0;
         for (char c : text) n_lines += c == '\n';
         std::string out((predict_tags ? 19 : 3) * text.size() + n_lines + 1, '\0');
         uint64_t n_out = 0, nl = 0;
         for (int attempt = 0; attempt < 2; ++attempt) {
             const int rc = predict_tags
-                ? vpt_tokenize_lines_tags(h_, reinterpret_cast<const uint8_t*>(text.data()), text.size(), no_norm ? 1 : 0,
-                                          wsconst_types, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl)
+                ? vpt_tokenize_lines_tags_rules(h_, detail::rules_handle(tag_rules), reinterpret_cast<const uint8_t*>(text.data()), text.size(), no_norm ? 1 : 0,
+                                                wsconst_types, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl)
                 : vpt_tokenize_lines(h_, reinterpret_cast<const uint8_t*>(text.data()), text.size(), no_norm ? 1 : 0,
                                      wsconst_types, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl);
             if (rc != 0 && attempt == 0 && n_out > out.size()) { out.assign(size_t(n_out) + 1, '\0'); continue; }  // long tag strings
@@ -380,6 +386,43 @@ private:
     bool tags_filled_ = false;
 };
 
+/// `vaporetto_rules::sentence_filters::PatternMatchTagger::new(rules)` for the tagged line path (`vpt_tag_rules_new`):
+/// surface -> one entry per tag slot (std::nullopt leaves the slot alone).  Fills the tag slots the model left None;
+/// unless no_norm, tokens are matched by their KyteaFullwidthFilter image and keys are not normalised.  Bound to the
+/// predictor, which must outlive it; it must outlive every call and stream that uses it.
+class TagRules {
+public:
+    TagRules(const Predictor& predictor, const std::vector<std::pair<std::string, std::vector<std::optional<std::string>>>>& rules) {
+        std::string surf, tags;
+        std::vector<uint64_t> soff{0}, qoff{0};
+        std::vector<uint32_t> slots;
+        for (const auto& r : rules) {
+            surf += r.first;
+            soff.push_back(surf.size());
+            for (const auto& t : r.second) {
+                slots.push_back(t ? uint32_t(tags.size()) : UINT32_MAX);
+                slots.push_back(t ? uint32_t(t->size()) : 0);
+                if (t) tags += *t;
+            }
+            qoff.push_back(slots.size() / 2);
+        }
+        detail::check(vpt_tag_rules_new(predictor.handle(), rules.size(), reinterpret_cast<const uint8_t*>(surf.data()),
+                                        soff.data(), qoff.data(), slots.data(), reinterpret_cast<const uint8_t*>(tags.data()),
+                                        tags.size(), &h_));
+    }
+    TagRules(const TagRules&) = delete;
+    TagRules& operator=(const TagRules&) = delete;
+    ~TagRules() { vpt_tag_rules_free(h_); }
+    const vpt_tag_rules* handle() const { return h_; }
+
+private:
+    vpt_tag_rules* h_ = nullptr;
+};
+
+namespace detail {
+inline const vpt_tag_rules* rules_handle(const TagRules* r) { return r ? r->handle() : nullptr; }
+}
+
 /// A line stream (`vpt_line_stream_*`): Predictor::tokenize_lines or evaluate_lines on input fed in pieces of any size,
 /// split at any byte, with host memory bounded by the pipeline rather than by the input.  The output goes to `sink` in
 /// input order as chunks complete, on the thread that calls feed / flush / finish; an exception thrown by the sink
@@ -388,11 +431,13 @@ class LineStream {
 public:
     using Sink = std::function<void(const uint8_t* bytes, size_t n)>;
     /// kind: VPT_STREAM_TOKENIZE (`sink` receives the tokenised lines) or VPT_STREAM_EVALUATE (`sink` may be empty).
+    /// tag_rules: as in Predictor::tokenize_lines.
     LineStream(const Predictor& predictor, int kind, Sink sink, bool no_norm = false, uint32_t wsconst_types = 0,
-               bool predict_tags = false)
+               bool predict_tags = false, const TagRules* tag_rules = nullptr)
         : sink_(std::move(sink)) {
-        detail::check(vpt_line_stream_new(predictor.handle(), kind, no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0,
-                                          sink_ ? &LineStream::write : nullptr, this, &h_));
+        detail::check(vpt_line_stream_new_rules(predictor.handle(), detail::rules_handle(tag_rules), kind, no_norm ? 1 : 0,
+                                                wsconst_types, predict_tags ? 1 : 0, sink_ ? &LineStream::write : nullptr,
+                                                this, &h_));
     }
     LineStream(const LineStream&) = delete;
     LineStream& operator=(const LineStream&) = delete;

@@ -10,7 +10,13 @@ input.  When nothing more is waiting on stdin, the output of every complete line
 an interactive session or a slow producer gets each line back as soon as it is entered, as with the reference.
 
 Options not on the device path (--scores, --tag-scores) are rejected; use the Sentence API
-(vaporetto_b200.Sentence / include/vaporetto_b200.hpp) for tags."""
+(vaporetto_b200.Sentence / include/vaporetto_b200.hpp) for tags.
+
+--tag-rules FILE is an extension: the reference CLI has no such option.  With --predict-tags it runs vaporetto_rules'
+PatternMatchTagger right after the tag prediction: every tag slot the model left empty for a token whose surface has
+a rule gets the rule's tag.  FILE holds one rule per line, written as one token of the tokenized format
+(Sentence::from_tokenized): `surface/tag1//tag3`, '\' escaping the next character; an empty tag field leaves its slot
+alone.  Unless --no-norm, tokens are matched by their full-width-normalised form, so write full-width surfaces."""
 import argparse
 import os
 import select
@@ -37,6 +43,43 @@ def read_model(path: str) -> bytes:
         return f.read()
 
 
+def parse_tag_rule(line: str, lineno: int):
+    """One line of a --tag-rules file -> (surface, [tag or None per slot]), as Sentence::from_tokenized reads a token
+    (sentence.rs:285-467): '\\' escapes the next character, '/' starts a tag, an empty tag is None.  A second token
+    (an unescaped ' ') or an empty surface is an error naming the line (1-based)."""
+    fields, cur, escape = [], [], False
+    for c in line:
+        if escape:
+            cur.append(c)
+            escape = False
+        elif c == "\\":
+            escape = True
+        elif c == "/":
+            fields.append("".join(cur))
+            cur = []
+        elif c == " ":
+            raise ValueError(f"--tag-rules line {lineno}: one token per line (found a space)")
+        else:
+            cur.append(c)
+    fields.append("".join(cur))
+    if not fields[0]:
+        raise ValueError(f"--tag-rules line {lineno}: empty surface")
+    return fields[0], [t if t else None for t in fields[1:]]
+
+
+def read_tag_rules(path: str) -> dict:
+    """The rules of a --tag-rules file (UTF-8, one rule per line; a line break ends a rule, '\\r\\n' included; a
+    surface given twice is an error, as a HashMap holds one entry per key)."""
+    rules = {}
+    with open(path, "rb") as f:
+        for i, raw in enumerate(f.read().decode("utf-8").splitlines(), 1):
+            surface, tags = parse_tag_rule(raw, i)
+            if surface in rules:
+                raise ValueError(f"--tag-rules line {i}: duplicate surface")
+            rules[surface] = tags
+    return rules
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description="A program to perform word segmentation (vaporetto_b200).")
     ap.add_argument("--model", required=True, help="The model file to use when analyzing text")
@@ -44,16 +87,29 @@ def main(argv=None) -> int:
                     help="Do not segment some character types: D Digit, R Roman, H Hiragana, T Katakana, K Kanji, O Other, G Grapheme cluster")
     ap.add_argument("--predict-tags", action="store_true", help="Predicts POS tags")
     ap.add_argument("--no-norm", action="store_true", help="Do not normalize input strings before prediction")
+    ap.add_argument("--tag-rules", metavar="FILE",
+                    help="Extension (not in the reference CLI): PatternMatchTagger rules, one `surface/tag1//tag3` per "
+                         "line, filling the tags the model leaves empty; needs --predict-tags")
     ap.add_argument("--device", type=int, default=0, help="CUDA device ordinal")
     args = ap.parse_args(argv)
+    if args.tag_rules and not args.predict_tags:
+        ap.error("--tag-rules needs --predict-tags")
+    rules = None
+    if args.tag_rules:
+        try:
+            rules = read_tag_rules(args.tag_rules)
+        except (ValueError, UnicodeDecodeError) as e:
+            ap.error(str(e))
 
     import vaporetto_b200 as vb
     print("Loading model file...", file=sys.stderr)
     predictor = vb.Predictor(vb.Model.read_zstd(read_model(args.model)), predict_tags=args.predict_tags, device=args.device)
+    tagger = vb.PatternMatchTagger(predictor, rules) if rules is not None else None
     print("Start tokenization", file=sys.stderr)
     inp, out = sys.stdin.buffer, sys.stdout.buffer
     t0 = time.perf_counter()
-    with predictor.line_stream(no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags) as stream:
+    with predictor.line_stream(no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
+                               tag_rules=tagger) as stream:
         while True:
             data = inp.read1(READ_BYTES)
             if not data:

@@ -13,7 +13,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 __all__ = ["Model", "Predictor", "Sentence", "VaporettoError", "CharacterBoundary", "CharacterType", "lib", "build",
-           "BatchResult", "build_blob", "shard_by_bytes", "LineStream", "SpansResult", "SpanToken", "Tokenizer"]
+           "BatchResult", "build_blob", "shard_by_bytes", "LineStream", "SpansResult", "SpanToken", "Tokenizer",
+           "PatternMatchTagger"]
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("VPT_B200_LIBRARY") or os.path.join(_PKG, "libvaporetto_b200.so")  # (override: A/B builds)
@@ -125,6 +126,12 @@ ABI = [
     ("vpt_line_stream_flush", C.c_int, [_P]),
     ("vpt_line_stream_finish", C.c_int, [_P, C.POINTER(C.c_uint64), _P]),
     ("vpt_line_stream_free", None, [_P]),
+    ("vpt_tag_rules_new", C.c_int, [_P, C.c_uint64, _P, _P, _P, _P, _P, C.c_uint64, C.POINTER(_P)]),
+    ("vpt_tag_rules_free", None, [_P]),
+    ("vpt_tag_rules_max_output", C.c_uint64, [_P]),
+    ("vpt_tokenize_lines_tags_rules", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, C.c_size_t,
+                                                C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("vpt_line_stream_new_rules", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
 ]
@@ -458,12 +465,14 @@ class Predictor:
                              None if cand is None else cand[: ntok.value * max(nt, 1)].reshape(-1, max(nt, 1)), int(nu.value))
 
     def tokenize_lines(self, data, out: Optional[np.ndarray] = None, no_norm: bool = False, wsconst: str = "",
-                       predict_tags: bool = False):
+                       predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None):
         """The reference CLI's `predict` loop (predict/src/main.rs:126-181) over a whole buffer of raw bytes
         (vpt_tokenize_lines): lines are split, scored (on KyteaFullwidthFilter(line) unless no_norm) and written
         out as space-separated tokens on the device; `wsconst`: letters of the CLI's --wsconst options ("D", "DR", ...:
         KyteaWsConstFilter; "G": ConcatGraphemeClustersFilter); `predict_tags`: the CLI's --predict-tags
-        (vpt_tokenize_lines_tags).  Returns (uint8 view of the output lines, number of lines)."""
+        (vpt_tokenize_lines_tags); `tag_rules`: a PatternMatchTagger made for this predictor, run after the tag
+        prediction (vpt_tokenize_lines_tags_rules; only with predict_tags).  Returns (uint8 view of the output lines,
+        number of lines)."""
         mask = _wsconst_mask(wsconst)
         t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
         if out is None:
@@ -471,6 +480,9 @@ class Predictor:
         n = C.c_uint64()
         nl = C.c_uint64()
         fn = lib().vpt_tokenize_lines_tags if predict_tags else lib().vpt_tokenize_lines
+        if tag_rules is not None and predict_tags:
+            def fn(h, *args, _rules=tag_rules._handle()):
+                return lib().vpt_tokenize_lines_tags_rules(h, _rules, *args)
         for _ in range(2):
             rc = fn(self._h, t.ctypes.data, t.size, int(no_norm), mask, out.ctypes.data, out.size, C.byref(n), C.byref(nl))
             if rc == 2 and predict_tags and n.value > out.size:
@@ -527,10 +539,11 @@ class Predictor:
                            None if cand is None else cand[: k * max(nt, 1)].reshape(-1, max(nt, 1))[:, :nt])
 
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
-                    predict_tags: bool = False) -> "LineStream":
+                    predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None) -> "LineStream":
         """tokenize_lines (kind="tokenize") or evaluate_lines (kind="evaluate") on input fed in pieces of any size,
-        with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream."""
-        return LineStream(self, kind, no_norm, wsconst, predict_tags)
+        with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream.  `tag_rules`
+        as in tokenize_lines."""
+        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules)
 
 
 class LineStream:
@@ -541,18 +554,21 @@ class LineStream:
     output of every complete line fed so far.  After an error every call raises it again.  Use as a context manager, or
     call close()."""
 
-    def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool):
+    def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool,
+                 tag_rules: Optional["PatternMatchTagger"] = None):
         if kind not in STREAM_KINDS:
             raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize' or 'evaluate'")
         mask = _wsconst_mask(wsconst)
         self._predictor = predictor  # (the stream uses the predictor until it is closed)
+        self._tag_rules = tag_rules  # (and the rules)
         self._kind = kind
         self._parts: List[bytes] = []
         self._exc: Optional[BaseException] = None
         self._write = STREAM_WRITE_FN(self._sink)  # (kept alive as long as the stream)
         h = _P()
-        _check(lib().vpt_line_stream_new(predictor._h, STREAM_KINDS[kind], int(no_norm), mask, int(predict_tags),
-                                         C.cast(self._write, _P), None, C.byref(h)))
+        rules = tag_rules._handle() if tag_rules is not None else None
+        _check(lib().vpt_line_stream_new_rules(predictor._h, rules, STREAM_KINDS[kind], int(no_norm), mask,
+                                               int(predict_tags), C.cast(self._write, _P), None, C.byref(h)))
         self._h = h
 
     def _sink(self, ctx, data, n):
@@ -601,6 +617,54 @@ class LineStream:
 
     def __exit__(self, *exc) -> None:
         self.close()
+
+    def __del__(self):
+        self.close()
+
+
+class PatternMatchTagger:
+    """`vaporetto_rules::sentence_filters::PatternMatchTagger::new(rules)` (pattern_match_tagger.rs:21-41) for the tagged
+    line path (vpt_tag_rules_new): `rules` maps a token surface to its tags, one entry per tag slot, None for a slot the
+    rule leaves alone.  Passed as `tag_rules=` to Predictor.tokenize_lines / line_stream with predict_tags, it fills
+    every tag slot the model left None for a token whose surface is a key; predicted tags are never overwritten.  Unless
+    no_norm, tokens are matched by their KyteaFullwidthFilter image and keys are not normalised: write full-width keys
+    ("ＡＢＣ") for the default, half-width ones match only with no_norm.  Bound to `predictor` (its device and n_tags)."""
+
+    def __init__(self, predictor: "Predictor", rules: dict):
+        surf, soff, qoff, slots, tags = bytearray(), [0], [0], [], bytearray()
+        for key, vals in rules.items():
+            surf += key.encode("utf-8")
+            soff.append(len(surf))
+            for v in vals:
+                if v is None:
+                    slots += [0xFFFFFFFF, 0]
+                else:
+                    b = v.encode("utf-8")
+                    slots += [len(tags), len(b)]
+                    tags += b
+            qoff.append(len(slots) // 2)
+        a = (np.frombuffer(bytes(surf) or b"\0", np.uint8), np.array(soff, np.uint64), np.array(qoff, np.uint64),
+             np.array(slots or [0], np.uint32), np.frombuffer(bytes(tags) or b"\0", np.uint8))  # (copied by the call)
+        self._predictor = predictor  # (the rules are bound to the predictor and must not outlive it)
+        self._h = None
+        h = _P()
+        _check(lib().vpt_tag_rules_new(predictor._h, len(rules), a[0].ctypes.data, a[1].ctypes.data, a[2].ctypes.data,
+                                       a[3].ctypes.data, a[4].ctypes.data, len(tags), C.byref(h)))
+        self._h = h
+
+    def _handle(self):
+        if self._h is None:
+            raise VaporettoError(2, "InvalidArgumentError: rules: closed")
+        return self._h
+
+    def max_output(self) -> int:
+        """The largest device output buffer a chunk of a call with these rules has used (vpt_tag_rules_max_output)."""
+        return int(lib().vpt_tag_rules_max_output(self._h)) if self._h else 0
+
+    def close(self) -> None:
+        h, self._h = getattr(self, "_h", None), None
+        if h and _lib is not None:
+            _lib.vpt_tag_rules_free(h)
 
     def __del__(self):
         self.close()

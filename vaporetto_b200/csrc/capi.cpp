@@ -3,6 +3,7 @@
 #include "../../include/vaporetto_b200.h"
 
 #include <algorithm>
+#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -23,6 +24,7 @@
 #include "model.hpp"
 #include "predictor_build.hpp"
 #include "grapheme.hpp"
+#include "tag_rules.hpp"
 #include "tags.hpp"
 #include "zstd_loader.hpp"
 #include "textnorm.hpp"
@@ -73,6 +75,7 @@ struct Scratch {
     void* d_toklocal = nullptr; size_t toklocal_cap = 0;
     void* d_tokblk = nullptr; size_t tokblk_cap = 0;
     void* d_ends = nullptr; size_t ends_cap = 0;   // token byte ends (vpt_token_spans)
+    void* d_trule = nullptr; size_t trule_cap = 0; // tag rules: the matched suffix sum (8 bytes), then a rule id per token
     // gold corpus and metrics (vpt_evaluate_lines)
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
@@ -89,7 +92,7 @@ struct Scratch {
     void* d_io = nullptr;          // its device twin
     ~Scratch() {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
-                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends,
+                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends, d_trule,
                         d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
@@ -137,6 +140,21 @@ struct vpt_predictor : HostPredictor {
             for (auto& b : pinned_pool) cudaFreeHost(b.first);
             cudaFree(d_blob);
             if (d_tags) cudaFree(d_tags);
+        }
+    }
+};
+
+// PatternMatchTagger rules on the predictor's device (tag_rules.hpp): one allocation holding all tables
+struct vpt_tag_rules {
+    const vpt_predictor* p = nullptr;
+    uint32_t n_rules = 0;
+    void* d_mem = nullptr;
+    DevTagRules dr;
+    mutable std::atomic<uint64_t> max_out{0};  // largest device output buffer of a chunk with these rules
+    ~vpt_tag_rules() {
+        if (d_mem) {
+            cudaSetDevice(p->device);
+            cudaFree(d_mem);
         }
     }
 };
@@ -987,6 +1005,7 @@ struct LineJob {
     uint32_t wsconst;  // post-filters (VPT_WSCONST_*)
     bool tags;         // tags predicted on the device
     int tag_mode;      // evaluate: how the system's tags compare with the gold's (kTags*)
+    const vpt_tag_rules* rules = nullptr;  // PatternMatchTagger after fill_tags (tokenize with tags and rules only)
 };
 
 // stage 0 of a chunk: H2D of its `nbytes` at `bytes`, newline counts, the number of lines to pinned host memory
@@ -1015,7 +1034,8 @@ void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* bytes) {
 // post-filters and, with `job.tags`, predicts the tags of every token into per-token records (the post-filters ran
 // first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
 // records; its output fields are left to the caller.
-TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job) {
+TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job,
+                      TagRuleArgs* ra = nullptr) {
     const bool normalize = job.normalize, tags = job.tags;
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
@@ -1104,6 +1124,14 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
         g.tok_work = static_cast<uint32_t*>(s.d_tokwork);
         g.norm = normalize ? 1 : 0;
         cuda_check(launch_tags(p.dt, g, st), "launch(tags)");
+        if (job.rules && ra) {
+            // the rule id of every token, and the sum of the matched rules' suffix bounds in front of them
+            Scratch::ensure(s.d_trule, s.trule_cap, 4 * nbytes + 16);
+            ra->rules = job.rules->dr;
+            ra->tok_rule = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(s.d_trule) + 8);
+            cuda_check(launch_rule_lookup(ra->rules, g, const_cast<int32_t*>(ra->tok_rule),
+                                          static_cast<unsigned long long*>(s.d_trule), st), "launch(rules)");
+        }
         t.tok_base = k.tok_base;
         t.tok_ids = g.tok_ids;
         t.tok_cands = g.tok_cands;
@@ -1147,19 +1175,30 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     const size_t ng = (n + kGroup - 1) / kGroup;
     // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
     // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
-    Scratch::ensure(s.d_out, s.out_cap, 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0));
+    const size_t out_need = 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0);
+    Scratch::ensure(s.d_out, s.out_cap, out_need);
     BatchArgs a;
     a.text = ch.sp.text;
     a.offsets = ch.sp.offsets;
     a.trims = ch.sp.trims;
     a.n_sent = n;
-    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job);
+    TagRuleArgs ra;
+    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job, &ra);
+    if (ra.tok_rule) {
+        // A rule's tag may be long on a short surface, so the rules' share of the output is sized from the suffixes the
+        // chunk's tokens actually matched: the host waits for the rule lookup and reads their sum.
+        cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
+        cuda_check(cudaStreamSynchronize(st), "sync(rules)");
+        Scratch::ensure(s.d_out, s.out_cap, out_need + size_t(s.h_totals[6]));
+        uint64_t seen = job.rules->max_out.load();
+        while (seen < s.out_cap && !job.rules->max_out.compare_exchange_weak(seen, s.out_cap)) {}
+    }
     t.tok_state = static_cast<uint64_t*>(s.d_tokg);
     t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
     t.total = t.tok_state + ng + 1;
     t.total_host = &s.h_totals[3];
     t.out = static_cast<uint8_t*>(s.d_out);
-    cuda_check(launch_tokenize(t, st), "launch(tok)");
+    cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
 }
@@ -1185,11 +1224,17 @@ bool check_lines_flags(const vpt_predictor* p, uint32_t wsconst_types, bool tags
     return tags;
 }
 
-LineJob line_job(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst_types, bool predict_tags) {
+LineJob line_job(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst_types, bool predict_tags,
+                 const vpt_tag_rules* rules = nullptr) {
     const bool tags = check_lines_flags(p, wsconst_types, predict_tags);
     // main.rs:110-120 with predictor.rs:553: the system keeps the gold tags (--no-norm) or has none, unless tags are
     // predicted with a model that has tag slots
-    return {kind, no_norm == 0, wsconst_types, tags, tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty};
+    LineJob j{kind, no_norm == 0, wsconst_types, tags, tags ? kTagsCompare : no_norm ? kTagsAlwaysEqual : kTagsGoldEmpty};
+    if (rules && rules->p != p)
+        throw Error(kInvalidArgument, "InvalidArgumentError: rules: made for another predictor");
+    // (rules act on predicted tags only: without them, or without any rule, the call is the one without rules)
+    if (rules && tags && kind == VPT_STREAM_TOKENIZE && rules->n_rules) j.rules = rules;
+    return j;
 }
 
 // Cuts a buffer of lines into pipeline chunks that end after a '\n' (memrchr from the nominal cut; a line longer than a
@@ -1478,9 +1523,10 @@ struct LineRing {
 };
 
 int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
-                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+                        uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out,
+                        const vpt_tag_rules* rules = nullptr) {
     VPT_API_BEGIN
-    const LineJob job = line_job(p, VPT_STREAM_TOKENIZE, no_norm, wsconst_types, tags);
+    const LineJob job = line_job(p, VPT_STREAM_TOKENIZE, no_norm, wsconst_types, tags, rules);
     if (out_len) *out_len = 0;
     if (n_lines_out) *n_lines_out = 0;
     if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
@@ -1518,6 +1564,57 @@ int vpt_tokenize_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_byt
 int vpt_tokenize_lines_tags(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
                             uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
     return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out);
+}
+
+int vpt_tag_rules_new(const vpt_predictor* p, uint64_t n_rules, const uint8_t* surfaces, const uint64_t* surface_offsets,
+                      const uint64_t* slot_offsets, const uint32_t* slots, const uint8_t* tags, uint64_t tags_len,
+                      vpt_tag_rules** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    if (!p) throw Error(kInvalidArgument, "InvalidArgumentError: predictor: must not be NULL");
+    const TagRulesHost t = build_tag_rules(n_rules, surfaces, surface_offsets, slot_offsets, slots, tags, tags_len,
+                                           uint32_t(p->n_tags));
+    require_device(p);
+    std::unique_ptr<vpt_tag_rules> r(new vpt_tag_rules());
+    r->p = p;
+    r->n_rules = t.n_rules;
+    const size_t sizes[6] = {t.tab.size() * sizeof(TagTokenEntry), t.surf.size(), t.slot_first.size() * 4,
+                             t.slot_ref.size() * 4, t.tag_bytes.size(), t.suffix.size() * 4};
+    const void* srcs[6] = {t.tab.data(), t.surf.data(), t.slot_first.data(), t.slot_ref.data(), t.tag_bytes.data(),
+                           t.suffix.data()};
+    size_t offs[6], total = 0;
+    for (int i = 0; i < 6; ++i) {
+        offs[i] = total;
+        total = align_up(total + sizes[i], 256);
+    }
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    cuda_check(cudaMalloc(&r->d_mem, total), "cudaMalloc(tag rules)");
+    uint8_t* base = static_cast<uint8_t*>(r->d_mem);
+    for (int i = 0; i < 6; ++i)
+        cuda_check(cudaMemcpy(base + offs[i], srcs[i], sizes[i], cudaMemcpyHostToDevice), "cudaMemcpy(tag rules)");
+    DevTagRules& d = r->dr;
+    d.tab = reinterpret_cast<const TagTokenEntry*>(base + offs[0]);
+    d.surf = base + offs[1];
+    d.slot_first = reinterpret_cast<const uint32_t*>(base + offs[2]);
+    d.slot_ref = reinterpret_cast<const uint2*>(base + offs[3]);
+    d.tag_bytes = base + offs[4];
+    d.suffix = reinterpret_cast<const uint32_t*>(base + offs[5]);
+    d.mask = t.mask;
+    d.max_bytes = t.max_bytes;
+    *out = r.release();
+    return kOk;
+    VPT_API_END
+}
+
+void vpt_tag_rules_free(vpt_tag_rules* rules) { delete rules; }
+
+uint64_t vpt_tag_rules_max_output(const vpt_tag_rules* rules) { return rules ? rules->max_out.load() : 0; }
+
+int vpt_tokenize_lines_tags_rules(const vpt_predictor* p, const vpt_tag_rules* rules, const uint8_t* utf8, size_t n_bytes,
+                                  int no_norm, uint32_t wsconst_types, uint8_t* out, size_t out_capacity, uint64_t* out_len,
+                                  uint64_t* n_lines_out) {
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out, rules);
 }
 
 int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
@@ -1689,12 +1786,18 @@ int stream_call(vpt_line_stream* st, const std::function<void()>& f) {
 
 int vpt_line_stream_new(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst_types, int predict_tags,
                         vpt_stream_write_fn write, void* ctx, vpt_line_stream** out) {
+    return vpt_line_stream_new_rules(p, nullptr, kind, no_norm, wsconst_types, predict_tags, write, ctx, out);
+}
+
+int vpt_line_stream_new_rules(const vpt_predictor* p, const vpt_tag_rules* rules, int kind, int no_norm,
+                              uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
+                              vpt_line_stream** out) {
     VPT_API_BEGIN
     if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
     *out = nullptr;
     if (kind != VPT_STREAM_TOKENIZE && kind != VPT_STREAM_EVALUATE)
         throw Error(kInvalidArgument, "InvalidArgumentError: kind: VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE");
-    const LineJob job = line_job(p, kind, no_norm, wsconst_types, predict_tags != 0);
+    const LineJob job = line_job(p, kind, no_norm, wsconst_types, predict_tags != 0, rules);
     if (kind == VPT_STREAM_TOKENIZE && !write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     *out = new vpt_line_stream(p, job, write, ctx);

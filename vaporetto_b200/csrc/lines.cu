@@ -17,6 +17,7 @@
 
 #include "device_model.hpp"
 #include "grapheme.hpp"
+#include "tag_rules.hpp"
 #include "textnorm.hpp"
 
 namespace vpt {
@@ -381,7 +382,13 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
 // that has a tag (an empty string for a slot without one), the strings escaped like the surface.  The suffix of the
 // token that ends in front of a character travels with that character's ' ' (it is written right before it); the last
 // token's suffix goes in front of the '\n'.  A token's record is tok_base[sentence] + (word boundaries before it).
-__device__ __forceinline__ uint32_t tag_suffix_len(const TokArgs& t, uint64_t rec) {
+// kRules: PatternMatchTagger's rules fill the slots the model left empty (tag_rules.hpp); without them the code is the
+// model-only writer.
+template <bool kRules>
+__device__ __forceinline__ uint32_t tag_suffix_len(const TokArgs& t, const TagRuleArgs& ra, uint64_t rec) {
+    if constexpr (kRules)
+        return merged_suffix_len(t.n_tags, t.tok_ids[rec], t.tok_cands + rec * t.n_tags, t.ts_slot, t.ts_cand, t.ts_ref,
+                                 ra.tok_rule[rec], ra.rules);
     const int32_t tid = t.tok_ids[rec];
     if (tid < 0) return 0;
     const uint32_t sb = __ldg(t.ts_slot + tid);
@@ -397,7 +404,13 @@ __device__ __forceinline__ uint32_t tag_suffix_len(const TokArgs& t, uint64_t re
     }
     return len;
 }
-__device__ __forceinline__ void tag_suffix_write(const TokArgs& t, uint64_t rec, uint8_t* __restrict__ out) {
+template <bool kRules>
+__device__ __forceinline__ void tag_suffix_write(const TokArgs& t, const TagRuleArgs& ra, uint64_t rec, uint8_t* __restrict__ out) {
+    if constexpr (kRules) {
+        merged_suffix_write(t.n_tags, t.tok_ids[rec], t.tok_cands + rec * t.n_tags, t.ts_slot, t.ts_cand, t.ts_ref,
+                            t.ts_bytes, ra.tok_rule[rec], ra.rules, out);
+        return;
+    }
     const int32_t tid = t.tok_ids[rec];
     if (tid < 0) return;
     const uint32_t sb = __ldg(t.ts_slot + tid);
@@ -414,8 +427,8 @@ __device__ __forceinline__ void tag_suffix_write(const TokArgs& t, uint64_t rec,
 }
 
 // One sentence by one warp: returns the output length without the '\n'; writes the bytes when kWrite.
-template <bool kWrite>
-__device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, uint64_t s, uint64_t o0, uint64_t o1, uint32_t trim, uint32_t nch,
+template <bool kWrite, bool kRules>
+__device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, const TagRuleArgs& ra, uint64_t s, uint64_t o0, uint64_t o1, uint32_t trim, uint32_t nch,
                                                     uint8_t* __restrict__ out, int lane) {
     const uint64_t a0 = o0 & ~3ull;
     const uint32_t b0 = uint32_t(o0 - a0), b1 = uint32_t(o1 - a0) - trim;
@@ -453,7 +466,7 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, uint64_t s
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 if (sp80 & (0x80u << (8 * j))) {
-                    sl[j] = tag_suffix_len(t, rec);
+                    sl[j] = tag_suffix_len<kRules>(t, ra, rec);
                     sl_sum += sl[j];
                     ++rec;
                 }
@@ -470,7 +483,7 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, uint64_t s
                 const uint32_t bit = 0x80u << (8 * j);
                 if (in80 & bit) {
                     if (sp80 & bit) {
-                        tag_suffix_write(t, rec, out + at);
+                        tag_suffix_write<kRules>(t, ra, rec, out + at);
                         at += sl[j];
                         ++rec;
                         out[at++] = 0x20;
@@ -487,14 +500,17 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, uint64_t s
     }
     uint32_t len = (b1 - b0) + extra;
     if (nch > 0) {
-        const uint32_t last = tag_suffix_len(t, rec0 + toks);
-        if (kWrite && lane == 0) tag_suffix_write(t, rec0 + toks, out + len);
+        const uint32_t last = tag_suffix_len<kRules>(t, ra, rec0 + toks);
+        if (kWrite && lane == 0) tag_suffix_write<kRules>(t, ra, rec0 + toks, out + len);
         len += last;
     }
     return len;
 }
 
-__global__ void __launch_bounds__(kTokThreads) k_tok_write_tags(TokArgs t, uint64_t ngroups) {
+// (kRules: one resident block per SM is enough for ptxas to keep the merge in registers; min blocks 0 is the bound
+// without a minimum, so the path without rules compiles as before)
+template <bool kRules>
+__global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags(TokArgs t, uint64_t ngroups, TagRuleArgs ra) {
     __shared__ uint64_t s_off[kGroup + 1];
     __shared__ uint32_t s_nch[kGroup], s_len[kGroup], s_excl[kGroup];
     __shared__ uint8_t s_trim[kGroup], s_bad[kGroup];
@@ -518,7 +534,7 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write_tags(TokArgs t, uint6
     // 1. output bytes per sentence
     for (int i = warp; i < ns; i += kTokThreads / 32) {
         uint32_t len = 1;  // the '\n'
-        if (!s_bad[i]) len += tagged_sentence<false>(t, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], nullptr, lane);
+        if (!s_bad[i]) len += tagged_sentence<false, kRules>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], nullptr, lane);
         if (lane == 0) s_len[i] = len;
     }
     __syncthreads();
@@ -565,7 +581,7 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write_tags(TokArgs t, uint6
     for (int i = warp; i < ns; i += kTokThreads / 32) {
         uint8_t* __restrict__ out = t.out + gout + s_excl[i];
         if (lane == 0) out[s_len[i] - 1] = 0x0A;
-        if (!s_bad[i]) tagged_sentence<true>(t, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], out, lane);
+        if (!s_bad[i]) tagged_sentence<true, kRules>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], out, lane);
     }
 }
 
@@ -779,13 +795,16 @@ cudaError_t launch_split_write(const SplitArgs& s, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-cudaError_t launch_tokenize(const TokArgs& t, cudaStream_t stream) {
+cudaError_t launch_tokenize(const TokArgs& t, cudaStream_t stream) { return launch_tokenize_rules(t, TagRuleArgs(), stream); }
+
+cudaError_t launch_tokenize_rules(const TokArgs& t, const TagRuleArgs& ra, cudaStream_t stream) {
     if (t.n_sent == 0) return cudaMemsetAsync(t.total, 0, 8, stream);
     const uint64_t ngroups = (t.n_sent + kGroup - 1) / kGroup;
     // look-back state words + the ticket that follows them
     cudaError_t e = cudaMemsetAsync(t.tok_state, 0, 8 * (ngroups + 1), stream);
     if (e != cudaSuccess) return e;
-    if (t.tok_base) k_tok_write_tags<<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups);
+    if (t.tok_base && ra.tok_rule) k_tok_write_tags<true><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra);
+    else if (t.tok_base) k_tok_write_tags<false><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra);
     else k_tok_write<<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups);
     return cudaGetLastError();
 }

@@ -13,6 +13,7 @@
 #include <atomic>
 
 #include "kernels_common.cuh"
+#include "tag_rules.hpp"
 #include "tags.hpp"
 #include "tags_token.hpp"
 
@@ -176,6 +177,25 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_score(DevTags t, TagArgs
     }
 }
 
+// PatternMatchTagger's rule lookup, one thread per token record, behind k_tok_lookup: every token is looked up, unknown
+// tokens included (they are what rules are for), by the surface bytes k_tok_lookup hashed.  A kernel of its own keeps
+// the path without rules as it was; the lookup costs one more pass over the descriptors and the token bytes.
+__global__ void __launch_bounds__(kTokTagThreads) k_rule_lookup(DevTagRules r, TagArgs a, int32_t* __restrict__ tok_rule,
+                                                                unsigned long long* __restrict__ suffix_sum) {
+    const uint64_t ntok = a.tok_base[a.n_sent];
+    const uint64_t stride = uint64_t(gridDim.x) * kTokTagThreads;
+    unsigned long long sum = 0;
+    for (uint64_t rec = uint64_t(blockIdx.x) * kTokTagThreads + threadIdx.x; rec < ntok; rec += stride) {
+        const uint4 d = a.tok_desc[rec];
+        const int32_t rid = rule_lookup(r, a.text + a.text_base + ((uint64_t(d.y & 0xFFFFu) << 32) | d.x), d.w, a.norm);
+        tok_rule[rec] = rid;
+        if (rid >= 0) sum += __ldg(r.suffix + rid);
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(kFull, sum, d);
+    if ((threadIdx.x & 31) == 0 && sum) atomicAdd(suffix_sum, sum);
+}
+
 // ---- compact outputs -----------------------------------------------------------------------------------------------------
 
 constexpr int kPackThreads = 256;
@@ -288,6 +308,18 @@ cudaError_t launch_compact(const CompactArgs& c, cudaStream_t stream) {
             k_token_base<<<unsigned((c.n_sent + kPackThreads - 1) / kPackThreads), kPackThreads, 0, stream>>>(c);
         }
     }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_rule_lookup(const DevTagRules& r, const TagArgs& a, int32_t* tok_rule, unsigned long long* suffix_sum,
+                               cudaStream_t stream) {
+    cudaError_t e = cudaMemsetAsync(suffix_sum, 0, sizeof *suffix_sum, stream);
+    if (e != cudaSuccess) return e;
+    if (a.n_sent == 0 || a.max_tokens == 0) return cudaSuccess;
+    if (!a.tok_desc || !a.tok_base) return cudaErrorInvalidValue;
+    // (grid-stride: the number of tokens is known on the device only; 2048 blocks fill an H100 at 16 per SM)
+    const uint64_t want = (a.max_tokens + kTokTagThreads - 1) / kTokTagThreads;
+    k_rule_lookup<<<unsigned(std::min<uint64_t>(want, 2048)), kTokTagThreads, 0, stream>>>(r, a, tok_rule, suffix_sum);
     return cudaGetLastError();
 }
 
