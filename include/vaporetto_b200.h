@@ -256,6 +256,9 @@ const char* vpt_tag_string(const vpt_predictor* predictor, uint32_t token_id, ui
 uint32_t vpt_tag_n_candidates(const vpt_predictor* predictor, uint32_t token_id, uint32_t slot);
 uint32_t vpt_tag_score_len(const vpt_predictor* predictor, uint32_t token_id);
 uint32_t vpt_tag_n_tokens(const vpt_predictor* predictor);
+/* number of tag slots of a token's own model (0 if out of range): `Token::tag_candidates` (sentence.rs:1219-1250) has one
+ * list per slot, empty slots included, which vpt_tag_n_candidates cannot tell from slots that do not exist */
+uint32_t vpt_tag_n_slots(const vpt_predictor* predictor, uint32_t token_id);
 
 /* predict (+ fill_tags) of a batch with COMPACT results, for callers that want the segmentation and the tags rather
  * than the score strip: what crosses PCIe is one bit per boundary and one small record per token.
@@ -280,6 +283,29 @@ int vpt_predict_batch_compact(const vpt_predictor* predictor, const uint8_t* utf
                               uint32_t* n_chars_out, uint8_t* status_out, uint32_t* n_tokens_out, int32_t* token_ids_out,
                               uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_boundaries_out,
                               uint64_t* n_tokens_total_out, uint64_t* n_unserved_out);
+/* Tag candidate scores (`Predictor::store_tag_scores(true)`, predictor.rs:511-514, as `Token::tag_candidates`,
+ * sentence.rs:1219-1250, reads them) of the batch, next to the token records of vpt_predict_batch_compact.  The other
+ * arguments and results are those of vpt_predict_batch_compact; tags are required (token_ids_out), and a predictor made
+ * with predict_tags = 0 gets its message.  With tag_scores_out == NULL the call IS vpt_predict_batch_compact.
+ *  - Which records.  A record gets scores exactly when its token_ids_out entry is >= 0.  Unknown tokens, tokens beyond the
+ *    device limits (counted in *n_unserved_out; vpt_fill_tags serves them with scores) and tokens whose model is
+ *    malformed (more candidates than scores: vpt_fill_tags reports InvalidModel) have id -1 and no scores.
+ *  - What.  The token's whole score vector, vpt_tag_score_len(token id) entries: its bias plus the char and type scorers'
+ *    tag weights, added with i32 wrap-around -- the `scores` predict_tags stores.  The candidate chosen for a slot with
+ *    two or more candidates is the first strict maximum of that slot's part of the vector (the parts follow each other in
+ *    slot order; slots with fewer than two candidates own no part).
+ *  - Layout.  The vectors of all records are concatenated in record order, with no gaps and no per-record offsets: the
+ *    vector of record r starts at the sum of vpt_tag_score_len(token_ids_out[q]) over the earlier records q with an id
+ *    >= 0.  The same input gives the same bytes.
+ *  - Capacity.  score_capacity is the number of int32 entries tag_scores_out holds; *n_scores_total_out receives the
+ *    total.  If it is too small the call returns VPT_INVALID_ARGUMENT with *n_scores_total_out set to the number needed.
+ *    An upper bound is token_capacity x the largest vpt_tag_score_len over the predictor's tokens. */
+int vpt_predict_batch_compact_tag_scores(const vpt_predictor* predictor, const uint8_t* utf8, const uint64_t* byte_offsets,
+                                         size_t n_sent, uint32_t* boundary_bits_out, size_t bits_capacity_words,
+                                         uint32_t* n_chars_out, uint8_t* status_out, uint32_t* n_tokens_out,
+                                         int32_t* token_ids_out, uint8_t* token_cands_out, size_t token_capacity,
+                                         uint64_t* n_boundaries_out, uint64_t* n_tokens_total_out, uint64_t* n_unserved_out,
+                                         int32_t* tag_scores_out, size_t score_capacity, uint64_t* n_scores_total_out);
 /* bits [first_bit, first_bit + n) of a boundary bit stream as bytes (0 / 1) */
 int vpt_unpack_boundaries(const uint32_t* boundary_bits, uint64_t first_bit, uint64_t n, uint8_t* boundaries_out);
 
@@ -527,6 +553,15 @@ int vpt_token_spans(const vpt_predictor* predictor, const uint8_t* utf8, const u
                     int32_t* token_ids_out,      /* nullable: tag prediction, as vpt_predict_batch_compact */
                     uint8_t* token_cands_out,    /* nullable: [token_capacity * n_tags] */
                     size_t token_capacity, uint64_t* n_tokens_total_out);
+/* vpt_token_spans with the tag candidate scores of every token record, under the contract of
+ * vpt_predict_batch_compact_tag_scores: the scores are those of the sentence that was tagged, i.e. of the pre-filtered
+ * text after the line-break and wsconst filters, where the tags come from.  A model with no tag slots gives id -1 for
+ * every token and no scores.  With tag_scores_out == NULL the call IS vpt_token_spans. */
+int vpt_token_spans_tag_scores(const vpt_predictor* predictor, const uint8_t* utf8, const uint64_t* byte_offsets,
+                               size_t n_docs, int no_norm, uint32_t wsconst_types, uint32_t* n_tokens_out,
+                               uint8_t* status_out, uint32_t* token_ends_out, int32_t* token_ids_out,
+                               uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_tokens_total_out,
+                               int32_t* tag_scores_out, size_t score_capacity, uint64_t* n_scores_total_out);
 
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */

@@ -14,6 +14,7 @@
 // Where the reference panics (fill_tags on a predictor created with predict_tags = false, predictor.rs:547-551)
 // this mirror throws VaporettoError(InvalidArgument).
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <exception>
 #include <functional>
@@ -177,6 +178,7 @@ public:
         std::vector<uint32_t> n_tokens;        // per sentence
         std::vector<int32_t> token_ids;        // per token (tags requested)
         std::vector<uint8_t> token_cands;      // per token x n_tags, 255 = none
+        std::vector<int32_t> tag_scores;       // score vectors of the tokens with id >= 0, record order (tag_scores requested)
         uint64_t n_boundaries = 0, n_unserved = 0;
         /// boundaries [first_bit, first_bit + n) as bytes (0 / 1)
         std::vector<uint8_t> boundaries(uint64_t first_bit, uint64_t n) const {
@@ -186,8 +188,10 @@ public:
         }
     };
     /// predict (+ predict_tags when `tags`) for a batch of sentences given as concatenated UTF-8 + byte offsets, with
-    /// compact results: one bit per boundary, one record per token.
-    CompactResult predict_batch_compact(const std::string& text, const std::vector<uint64_t>& byte_offsets, bool tags = false) const {
+    /// compact results: one bit per boundary, one record per token; `tag_scores` (with `tags`): the tag candidate scores
+    /// of the records too (`vpt_predict_batch_compact_tag_scores`).
+    CompactResult predict_batch_compact(const std::string& text, const std::vector<uint64_t>& byte_offsets, bool tags = false,
+                                        bool tag_scores = false) const {
         CompactResult r;
         const size_t n = byte_offsets.empty() ? 0 : byte_offsets.size() - 1;
         const size_t cap = text.size() + 1;
@@ -197,15 +201,17 @@ public:
         r.n_tokens.assign(n, 0);
         const size_t nt = tags ? size_t(info_.n_tags) : 0;
         if (tags) { r.token_ids.assign(cap, -1); r.token_cands.assign(cap * (nt ? nt : 1), 255); }
-        uint64_t ntok = 0;
+        uint64_t ntok = 0, nsc = 0;
+        if (tag_scores) r.tag_scores.assign(std::max<size_t>(cap * max_score_len(), 1), 0);
         if (n)
-            detail::check(vpt_predict_batch_compact(h_, reinterpret_cast<const uint8_t*>(text.data()), byte_offsets.data(), n,
-                                                    r.boundary_bits.data(), r.boundary_bits.size(), r.n_chars.data(), r.status.data(),
-                                                    r.n_tokens.data(), tags ? r.token_ids.data() : nullptr,
-                                                    tags ? r.token_cands.data() : nullptr, tags ? cap : 0, &r.n_boundaries, &ntok,
-                                                    &r.n_unserved));
+            detail::check(vpt_predict_batch_compact_tag_scores(
+                h_, reinterpret_cast<const uint8_t*>(text.data()), byte_offsets.data(), n, r.boundary_bits.data(),
+                r.boundary_bits.size(), r.n_chars.data(), r.status.data(), r.n_tokens.data(), tags ? r.token_ids.data() : nullptr,
+                tags ? r.token_cands.data() : nullptr, tags ? cap : 0, &r.n_boundaries, &ntok, &r.n_unserved,
+                tag_scores ? r.tag_scores.data() : nullptr, r.tag_scores.size(), &nsc));
         r.boundary_bits.resize(size_t((r.n_boundaries + 31) / 32));
         if (tags) { r.token_ids.resize(size_t(ntok)); r.token_cands.resize(size_t(ntok) * (nt ? nt : 1)); }
+        r.tag_scores.resize(size_t(nsc));
         return r;
     }
 
@@ -217,6 +223,7 @@ public:
         std::vector<uint32_t> token_ends;      // per token: exclusive end, in bytes from its document's start
         std::vector<int32_t> token_ids;        // per token (tags requested)
         std::vector<uint8_t> token_cands;      // per token x n_tags, 255 = none
+        std::vector<int32_t> tag_scores;       // score vectors of the tokens with id >= 0, record order (tag_scores requested)
         /// [from, to) byte offsets of token r of document d
         std::pair<uint32_t, uint32_t> span(size_t d, size_t r) const {
             const size_t i = size_t(token_base[d]) + r;
@@ -227,7 +234,7 @@ public:
     /// byte offsets: the full-width pre-filter (unless `no_norm`), predict, the line-break split and the `wsconst_types`
     /// post-filters on the device; the token byte spans (+ tag records when `tags`) come back.
     SpansResult token_spans(const std::string& text, const std::vector<uint64_t>& byte_offsets, bool no_norm = false,
-                            uint32_t wsconst_types = 0, bool tags = false) const {
+                            uint32_t wsconst_types = 0, bool tags = false, bool tag_scores = false) const {
         SpansResult r;
         const size_t n = byte_offsets.empty() ? 0 : byte_offsets.size() - 1;
         const size_t cap = text.size() + 1;  // a token has at least one byte
@@ -236,17 +243,27 @@ public:
         r.token_ends.assign(cap, 0);
         const size_t nt = tags ? size_t(info_.n_tags) : 0;
         if (tags) { r.token_ids.assign(cap, -1); r.token_cands.assign(cap * (nt ? nt : 1), 255); }
-        uint64_t ntok = 0;
+        uint64_t ntok = 0, nsc = 0;
+        if (tag_scores) r.tag_scores.assign(std::max<size_t>(cap * max_score_len(), 1), 0);
         if (n)
-            detail::check(vpt_token_spans(h_, reinterpret_cast<const uint8_t*>(text.data()), byte_offsets.data(), n,
-                                          no_norm ? 1 : 0, wsconst_types, r.n_tokens.data(), r.status.data(),
-                                          r.token_ends.data(), tags ? r.token_ids.data() : nullptr,
-                                          tags ? r.token_cands.data() : nullptr, cap, &ntok));
+            detail::check(vpt_token_spans_tag_scores(h_, reinterpret_cast<const uint8_t*>(text.data()), byte_offsets.data(), n,
+                                                     no_norm ? 1 : 0, wsconst_types, r.n_tokens.data(), r.status.data(),
+                                                     r.token_ends.data(), tags ? r.token_ids.data() : nullptr,
+                                                     tags ? r.token_cands.data() : nullptr, cap, &ntok,
+                                                     tag_scores ? r.tag_scores.data() : nullptr, r.tag_scores.size(), &nsc));
         r.token_ends.resize(size_t(ntok));
+        r.tag_scores.resize(size_t(nsc));
         if (tags) { r.token_ids.resize(size_t(ntok)); r.token_cands.resize(size_t(ntok) * nt); }
         r.token_base.assign(n + 1, 0);
         for (size_t d = 0; d < n; ++d) r.token_base[d + 1] = r.token_base[d] + r.n_tokens[d];
         return r;
+    }
+
+    /// the longest tag score vector of the predictor's tokens (vpt_tag_score_len)
+    size_t max_score_len() const {
+        size_t m = 0;
+        for (uint32_t t = 0, n = vpt_tag_n_tokens(h_); t < n; ++t) m = std::max<size_t>(m, vpt_tag_score_len(h_, t));
+        return m;
     }
 
     const vpt_predictor_info& info() const { return info_; }

@@ -10,7 +10,10 @@ input.  When nothing more is waiting on stdin, the output of every complete line
 an interactive session or a slow producer gets each line back as soon as it is entered, as with the reference.
 
 Options not on the device path (--scores, --tag-scores) are rejected; use the Sentence API
-(vaporetto_b200.Sentence / include/vaporetto_b200.hpp) for tags.
+(vaporetto_b200.Sentence / include/vaporetto_b200.hpp) for tags.  For the tag candidate scores --tag-scores prints, call
+the library: Predictor.predict_batch_compact(..., tags=True, tag_scores=True) or Predictor.token_spans(..., tags=True,
+tag_scores=True) and the result's tag_candidates(r) for a batch, Predictor.store_tag_scores(True) + Token.tag_candidates()
+for one sentence (C: vpt_predict_batch_compact_tag_scores, vpt_token_spans_tag_scores).
 
 --tag-rules FILE is an extension: the reference CLI has no such option.  With --predict-tags it runs vaporetto_rules'
 PatternMatchTagger right after the tag prediction: every tag slot the model left empty for a token whose surface has

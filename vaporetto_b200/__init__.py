@@ -134,6 +134,12 @@ ABI = [
     ("vpt_line_stream_new_rules", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
+    ("vpt_tag_n_slots", C.c_uint32, [_P, C.c_uint32]),
+    ("vpt_predict_batch_compact_tag_scores", C.c_int, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _P, _P, _P, _P, _P,
+                                                       C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                                       C.POINTER(C.c_uint64), _P, C.c_size_t, C.POINTER(C.c_uint64)]),
+    ("vpt_token_spans_tag_scores", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
+                                             C.POINTER(C.c_uint64), _P, C.c_size_t, C.POINTER(C.c_uint64)]),
 ]
 
 # vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
@@ -341,6 +347,27 @@ class Predictor:
         self.info = {k: getattr(info, k) for k, _ in _Info._fields_}
         self.n_tags = info.n_tags
         self.predict_tags = bool(info.predict_tags)
+        self._store_tag_scores = False
+        self._score_len_table = None
+
+    def store_tag_scores(self, flag: bool) -> None:
+        """`Predictor::store_tag_scores(flag)` (predictor.rs:511-514): Sentence.fill_tags keeps every known token's score
+        vector, for Token.tag_candidates."""
+        self._store_tag_scores = bool(flag)
+
+    def _score_lens(self) -> np.ndarray:
+        """vpt_tag_score_len of every token id (int64), built once per predictor."""
+        if self._score_len_table is None:
+            L = lib()
+            n = L.vpt_tag_n_tokens(self._h)
+            self._score_len_table = np.array([L.vpt_tag_score_len(self._h, t) for t in range(n)], np.int64)
+        return self._score_len_table
+
+    def tag_candidates(self, token_id: int, scores) -> list:
+        """`Token::tag_candidates` (sentence.rs:1219-1250) of a token with id `token_id` (-1: none) and score vector
+        `scores`: one list of (tag, score) per tag slot of the token's own model; a slot with one candidate gives
+        (tag, 0), an empty slot gives []."""
+        return _tag_candidates(self, token_id, scores)
 
     def kernel_plan(self, states: bool = False) -> dict:
         """The scoring kernel a batch runs (`kernel`: k_fused, k_tile_fast, k_score_fast or k_score_general), its
@@ -383,6 +410,7 @@ class Predictor:
         sentence._type_states = ts
         sentence._predictor = self
         sentence._tags = None
+        sentence._tag_scores = None
 
     def predict_batch(self, text, offsets, want_scores: bool = True, want_states: bool = False,
                       out: Optional[BatchResult] = None) -> BatchResult:
@@ -442,9 +470,12 @@ class Predictor:
         v = lib().vpt_tag_string(self._h, int(token_id), int(slot), int(cand))
         return None if v is None else v.decode("utf-8")
 
-    def predict_batch_compact(self, text, offsets, tags: bool = False) -> "CompactResult":
+    def predict_batch_compact(self, text, offsets, tags: bool = False, tag_scores: bool = False) -> "CompactResult":
         """predict (+ predict_tags) for a batch with compact results (vpt_predict_batch_compact): one bit per boundary, one
-        record per token; see CompactResult."""
+        record per token; see CompactResult.  `tag_scores` (with tags): the tag candidate scores of every token record too
+        (vpt_predict_batch_compact_tag_scores; CompactResult.tag_candidates)."""
+        if tag_scores and not tags:
+            raise VaporettoError(2, "InvalidArgumentError: tag_scores: needs tags=True")
         t = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text, np.uint8)
         off = np.ascontiguousarray(offsets, np.uint64)
         n = off.size - 1
@@ -457,12 +488,22 @@ class Predictor:
         tok = np.empty(cap, np.int32) if tags else None
         cand = np.empty(cap * max(nt, 1), np.uint8) if tags else None
         nb, ntok, nu = C.c_uint64(), C.c_uint64(), C.c_uint64()
-        _check(lib().vpt_predict_batch_compact(self._h, t.ctypes.data, off.ctypes.data, n, bits.ctypes.data, bits.size,
-                                               n_chars.ctypes.data, status.ctypes.data, n_tokens.ctypes.data, _ptr(tok), _ptr(cand),
-                                               cap if tags else 0, C.byref(nb), C.byref(ntok), C.byref(nu)))
-        return CompactResult(bits[: (nb.value + 31) // 32], int(nb.value), n_chars[:n], status[:n], n_tokens[:n],
-                             None if tok is None else tok[: ntok.value],
-                             None if cand is None else cand[: ntok.value * max(nt, 1)].reshape(-1, max(nt, 1)), int(nu.value))
+        sc, nsc = self._score_buffer(cap) if tag_scores else None, C.c_uint64()
+        _check(lib().vpt_predict_batch_compact_tag_scores(
+            self._h, t.ctypes.data, off.ctypes.data, n, bits.ctypes.data, bits.size, n_chars.ctypes.data, status.ctypes.data,
+            n_tokens.ctypes.data, _ptr(tok), _ptr(cand), cap if tags else 0, C.byref(nb), C.byref(ntok), C.byref(nu), _ptr(sc),
+            0 if sc is None else sc.size, C.byref(nsc)))
+        r = CompactResult(bits[: (nb.value + 31) // 32], int(nb.value), n_chars[:n], status[:n], n_tokens[:n],
+                          None if tok is None else tok[: ntok.value],
+                          None if cand is None else cand[: ntok.value * max(nt, 1)].reshape(-1, max(nt, 1)), int(nu.value))
+        if tag_scores:
+            _attach_scores(r, self, sc[: nsc.value])
+        return r
+
+    def _score_buffer(self, max_tokens: int) -> np.ndarray:
+        """int32 buffer for the tag scores of at most `max_tokens` token records (each gets at most the longest vector)."""
+        lens = self._score_lens()
+        return np.empty(max(max_tokens * int(lens.max(initial=0)), 1), np.int32)
 
     def tokenize_lines(self, data, out: Optional[np.ndarray] = None, no_norm: bool = False, wsconst: str = "",
                        predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None):
@@ -514,11 +555,15 @@ class Predictor:
         out = {name: int(getattr(counts, name)) for name, _ in _EvalCounts._fields_}
         return (out, lc) if per_line else out
 
-    def token_spans(self, text, offsets, no_norm: bool = False, wsconst: str = "", tags: bool = False) -> "SpansResult":
+    def token_spans(self, text, offsets, no_norm: bool = False, wsconst: str = "", tags: bool = False,
+                    tag_scores: bool = False) -> "SpansResult":
         """vaporetto_tantivy's token_stream (lib.rs:157-229) for a batch of documents on the device (vpt_token_spans):
         document d is text[offsets[d]:offsets[d + 1]] (bytes or uint8 array, UTF-8); it is pre-filtered (unless
         `no_norm`), predicted, split on both sides of every '\r' / '\n' and post-filtered by the `wsconst` letters
-        (D, R, H, T, K, O, G).  `tags`: the tag records of every token (needs predict_tags).  See SpansResult."""
+        (D, R, H, T, K, O, G).  `tags`: the tag records of every token (needs predict_tags).  `tag_scores` (with tags):
+        their tag candidate scores too (vpt_token_spans_tag_scores; SpansResult.tag_candidates).  See SpansResult."""
+        if tag_scores and not tags:
+            raise VaporettoError(2, "InvalidArgumentError: tag_scores: needs tags=True")
         mask = _wsconst_mask(wsconst)
         t = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray)) else np.ascontiguousarray(text, np.uint8)
         off = np.ascontiguousarray(offsets, np.uint64)
@@ -531,12 +576,17 @@ class Predictor:
         tok = np.empty(cap, np.int32) if tags else None
         cand = np.empty(cap * max(nt, 1), np.uint8) if tags else None
         total = C.c_uint64()
-        _check(lib().vpt_token_spans(self._h, t.ctypes.data, off.ctypes.data, max(n, 0), int(no_norm), mask,
-                                     n_tokens.ctypes.data, status.ctypes.data, ends.ctypes.data, _ptr(tok), _ptr(cand),
-                                     cap, C.byref(total)))
+        sc, nsc = self._score_buffer(cap) if tag_scores else None, C.c_uint64()
+        _check(lib().vpt_token_spans_tag_scores(self._h, t.ctypes.data, off.ctypes.data, max(n, 0), int(no_norm), mask,
+                                                n_tokens.ctypes.data, status.ctypes.data, ends.ctypes.data, _ptr(tok),
+                                                _ptr(cand), cap, C.byref(total), _ptr(sc), 0 if sc is None else sc.size,
+                                                C.byref(nsc)))
         k = int(total.value)
-        return SpansResult(n_tokens[:max(n, 0)], status[:max(n, 0)], ends[:k], None if tok is None else tok[:k],
-                           None if cand is None else cand[: k * max(nt, 1)].reshape(-1, max(nt, 1))[:, :nt])
+        r = SpansResult(n_tokens[:max(n, 0)], status[:max(n, 0)], ends[:k], None if tok is None else tok[:k],
+                        None if cand is None else cand[: k * max(nt, 1)].reshape(-1, max(nt, 1))[:, :nt])
+        if tag_scores:
+            _attach_scores(r, self, sc[: nsc.value])
+        return r
 
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None) -> "LineStream":
@@ -685,7 +735,47 @@ def _wsconst_mask(wsconst: str) -> int:
     return mask
 
 
-class CompactResult:
+def _tag_candidates(p: "Predictor", token_id: int, scores) -> list:
+    """Token::tag_candidates (sentence.rs:1219-1250) over the predictor's tag strings."""
+    if token_id < 0:
+        return []
+    L = lib()
+    out, i = [], 0
+    for k in range(L.vpt_tag_n_slots(p._h, token_id)):
+        nc = L.vpt_tag_n_candidates(p._h, token_id, k)
+        tag = lambda c: L.vpt_tag_string(p._h, token_id, k, c).decode("utf-8")
+        if nc == 1:
+            out.append([(tag(0), 0)])
+        else:
+            out.append([(tag(c), int(scores[i + c])) for c in range(nc)])
+            i += nc
+    return out
+
+
+def _attach_scores(r, p: "Predictor", scores: np.ndarray) -> None:
+    """tag_scores, score_offsets and the predictor behind tag_candidates of a CompactResult / SpansResult."""
+    ids = r.token_ids
+    lens = np.append(p._score_lens(), 0)[ids]  # (id -1: the appended 0)
+    r.tag_scores = scores
+    r.score_offsets = np.concatenate(([0], np.cumsum(lens))).astype(np.uint64)
+    r._predictor = p
+
+
+class _ScoredRecords:
+    """tag_candidates of the token records of a result with tag scores."""
+    tag_scores = None       # int32: the score vectors of the records with a token id >= 0, in record order
+    score_offsets = None    # uint64 [tokens + 1]: record r's vector is tag_scores[score_offsets[r]:score_offsets[r + 1]]
+
+    def tag_candidates(self, r: int) -> list:
+        """`Token::tag_candidates` of token record r: [[(tag, score), ...] per tag slot]; a one-candidate slot gives
+        (tag, 0), an empty slot [], a record with id -1 []."""
+        if self.tag_scores is None:
+            raise VaporettoError(2, "InvalidArgumentError: tag_candidates: the call was made without tag_scores=True")
+        lo, hi = int(self.score_offsets[r]), int(self.score_offsets[r + 1])
+        return _tag_candidates(self._predictor, int(self.token_ids[r]), self.tag_scores[lo:hi])
+
+
+class CompactResult(_ScoredRecords):
     """Result of Predictor.predict_batch_compact: `boundary_bits` (uint32 words of the batch's boundary bit stream),
     `n_chars` / `status` / `n_tokens` per sentence, `token_ids` [tokens] and `token_cands` [tokens, n_tags] (uint8, 255 =
     none) when tags were requested.  Sentence s owns the bits [bit_offsets[s], bit_offsets[s + 1]) and the token records
@@ -707,7 +797,7 @@ class CompactResult:
         return out
 
 
-class SpansResult:
+class SpansResult(_ScoredRecords):
     """Result of Predictor.token_spans: `n_tokens` and `status` (VPT_SENT_*: 0 ok, 1 empty, 2 NUL, 3 invalid UTF-8) per
     document, `token_base` (n_docs + 1, uint64) the first token record of every document, `token_ends` (uint32) the byte
     offset of every token's exclusive end from its document's start, and with tags `token_ids` (int32, -1: no tag model)
@@ -802,6 +892,16 @@ class Token:
         k = self._s.n_tags()
         return self._s.tags()[(self._end - 1) * k:self._end * k]
 
+    def tag_candidates(self):
+        """`Token::tag_candidates` (sentence.rs:1219-1250): [[(tag, score), ...] per tag slot of the token's model]; []
+        for a token without a tag model.  Needs Predictor.store_tag_scores(True) before fill_tags (the reference
+        panics without it)."""
+        s = self._s
+        if s._tag_scores is None:
+            raise RuntimeError("Predictor::store_tag_scores() must be set to true to use this function.")
+        i = self._end - 1
+        return _tag_candidates(s._predictor, int(s._tag_token[i]), s._tag_scores[i])
+
 
 class Sentence:
     """`vaporetto::Sentence` (sentence.rs:85-1193), raw-text subset used around `predict`."""
@@ -840,6 +940,7 @@ class Sentence:
         self._tags = None
         self._tag_token = None
         self._tag_cand = None
+        self._tag_scores = None
 
     def as_raw_text(self) -> str:
         return self._bytes.decode("utf-8")
@@ -882,10 +983,15 @@ class Sentence:
         k = p.n_tags
         tt = np.full(self._n, -1, np.int32)
         tc = np.full(max(self._n * k, 1), -1, np.int32)
+        ts = None
+        if p._store_tag_scores:
+            stride = max(int(p._score_lens().max(initial=0)), 1)
+            ts = np.zeros((self._n, stride), np.int32)
         _check(lib().vpt_fill_tags(p._h, self._bytes, len(self._bytes), self._boundaries.ctypes.data,
                                    _ptr(self._char_states), _ptr(self._type_states), tt.ctypes.data, tc.ctypes.data,
-                                   None, 0))
+                                   _ptr(ts), 0 if ts is None else ts.shape[1]))
         self._tag_token, self._tag_cand = tt, tc
+        self._tag_scores = None if ts is None else [ts[i, : p._score_lens()[t]] if t >= 0 else ts[i, :0] for i, t in enumerate(tt)]
         tags: List[Optional[str]] = []
         for i in range(self._n):
             for s in range(k):

@@ -76,6 +76,9 @@ struct Scratch {
     void* d_tokblk = nullptr; size_t tokblk_cap = 0;
     void* d_ends = nullptr; size_t ends_cap = 0;   // token byte ends (vpt_token_spans)
     void* d_trule = nullptr; size_t trule_cap = 0; // tag rules: the matched suffix sum (8 bytes), then a rule id per token
+    void* d_scoff = nullptr; size_t scoff_cap = 0; // tag candidate scores (TagScoreArgs): per-record counts / offsets,
+    void* d_scblk = nullptr; size_t scblk_cap = 0; // block totals / prefix,
+    void* d_tagsc = nullptr; size_t tagsc_cap = 0; // the chunk's score vectors
     // gold corpus and metrics (vpt_evaluate_lines)
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
@@ -86,13 +89,15 @@ struct Scratch {
     void* d_lc = nullptr; size_t lc_cap = 0;
     void* d_evtot = nullptr; size_t evtot_cap = 0;
     uint64_t* h_eval = nullptr;    // pinned, kEvalTotals + 1 x u64: a chunk's totals and error key
-    uint64_t* h_totals = nullptr;  // pinned, 8 x u64: boundaries, chars, lines, output bytes, tokens, first bit word
+    uint64_t* h_totals = nullptr;  // pinned, 8 x u64: boundaries, chars, lines, output bytes, tokens, first bit word, rule
+                                   // suffix bytes, tag scores
     uint32_t* h_side = nullptr; size_t side_cap = 0;  // pinned: first bit word of every chunk (vpt_predict_batch_compact)
     uint8_t* h_io = nullptr;       // pinned staging of the single-sentence call (vpt_predict), kSingleIoBytes
     void* d_io = nullptr;          // its device twin
     ~Scratch() {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
                         d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends, d_trule,
+                        d_scoff, d_scblk, d_tagsc,
                         d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
@@ -2004,6 +2009,11 @@ uint32_t vpt_tag_n_candidates(const vpt_predictor* p, uint32_t token_id, uint32_
     return slot < t.size() ? uint32_t(t[slot].size()) : 0;
 }
 
+uint32_t vpt_tag_n_slots(const vpt_predictor* p, uint32_t token_id) {
+    if (!p || token_id >= p->tag_preds.size()) return 0;
+    return uint32_t(p->tag_preds[token_id].tags.size());
+}
+
 uint32_t vpt_tag_score_len(const vpt_predictor* p, uint32_t token_id) {
     if (!p || token_id >= p->tag_preds.size()) return 0;
     return uint32_t(p->tag_preds[token_id].bias.size());
@@ -2141,18 +2151,59 @@ int vpt_predict_batch_tags(const vpt_predictor* p, const uint8_t* utf8, const ui
     VPT_API_END
 }
 
+namespace {
+
+// The longest score vector k_tok_score stores for a token of this predictor: the device path serves tokens of at most
+// kTagMaxScores scores.  A chunk of `nc` characters has at most nc token records, so nc x this bounds its scores.
+size_t device_score_len_bound(const vpt_predictor* p) {
+    size_t m = 0;
+    for (const TagPredictorHost& tp : p->tag_preds) m = std::max(m, tp.bias.size());
+    return std::min<size_t>(m, size_t(kTagMaxScores));
+}
+
+// Scratch of the tag candidate scores of one chunk of at most `nc` token records; its total arrives in h_totals[7].
+TagScoreArgs bind_tag_scores(Scratch& s, uint64_t nc, size_t len_bound) {
+    Scratch::ensure(s.d_scoff, s.scoff_cap, 4 * nc + 16);
+    Scratch::ensure(s.d_scblk, s.scblk_cap, 8 * (nc / kScoreScanBlock + 4));
+    Scratch::ensure(s.d_tagsc, s.tagsc_cap, 4 * nc * len_bound + 16);
+    TagScoreArgs sc;
+    sc.rec_off = static_cast<uint32_t*>(s.d_scoff);
+    sc.blk = static_cast<uint64_t*>(s.d_scblk);
+    sc.scores = static_cast<int32_t*>(s.d_tagsc);
+    s.h_totals[7] = 0;
+    sc.total_host = &s.h_totals[7];
+    return sc;
+}
+
+}  // namespace
+
 int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_sent,
                               uint32_t* boundary_bits_out, size_t bits_capacity_words, uint32_t* n_chars_out,
                               uint8_t* status_out, uint32_t* n_tokens_out, int32_t* token_ids_out, uint8_t* token_cands_out,
                               size_t token_capacity, uint64_t* n_boundaries_out, uint64_t* n_tokens_total_out,
                               uint64_t* n_unserved_out) {
+    return vpt_predict_batch_compact_tag_scores(p, utf8, byte_offsets, n_sent, boundary_bits_out, bits_capacity_words, n_chars_out,
+                                                status_out, n_tokens_out, token_ids_out, token_cands_out, token_capacity,
+                                                n_boundaries_out, n_tokens_total_out, n_unserved_out, nullptr, 0, nullptr);
+}
+
+int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_sent,
+                                         uint32_t* boundary_bits_out, size_t bits_capacity_words, uint32_t* n_chars_out,
+                                         uint8_t* status_out, uint32_t* n_tokens_out, int32_t* token_ids_out,
+                                         uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_boundaries_out,
+                                         uint64_t* n_tokens_total_out, uint64_t* n_unserved_out, int32_t* tag_scores_out,
+                                         size_t score_capacity, uint64_t* n_scores_total_out) {
     VPT_API_BEGIN
     require_device(p);
     if (n_boundaries_out) *n_boundaries_out = 0;
     if (n_tokens_total_out) *n_tokens_total_out = 0;
     if (n_unserved_out) *n_unserved_out = 0;
+    if (n_scores_total_out) *n_scores_total_out = 0;
     const bool want_tags = token_ids_out != nullptr || token_cands_out != nullptr;
     const bool want_tokens = want_tags || n_tokens_out != nullptr;
+    const bool want_scores = tag_scores_out != nullptr;
+    if (want_scores && !want_tags)
+        throw Error(kInvalidArgument, "InvalidArgumentError: tag_scores_out: needs token_ids_out (tag prediction)");
     if (want_tags) {
         if (!p->predict_tags || p->from_blob)
             throw Error(kInvalidArgument, "InvalidArgumentError: this predictor is created with predict_tags = false");
@@ -2202,7 +2253,8 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
         ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
     }
     const size_t nt = want_tags ? p->n_tags : 0;
-    uint64_t nb_total = 0, tok_total = 0, unserved_total = 0;
+    const size_t score_len = want_scores ? device_score_len_bound(p) : 0;
+    uint64_t nb_total = 0, tok_total = 0, unserved_total = 0, score_total = 0;
     bool overflow = false;
     // pinned words that receive every chunk's first bit word (merged into the output at the end)
     Scratch& s0 = *lease[0]->s;
@@ -2296,7 +2348,12 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
             Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * cc.nc + 32);
             t.tok_work = static_cast<uint32_t*>(s.d_tokwork);
             t.text_base = 0;
-            cuda_check(launch_tags(p->dt, t, st), "launch(tags)");
+            if (want_scores) {
+                const TagScoreArgs sc = bind_tag_scores(s, cc.nc, score_len);
+                cuda_check(launch_tags(p->dt, t, st, &sc), "launch(tags)");
+            } else {
+                cuda_check(launch_tags(p->dt, t, st), "launch(tags)");
+            }
             cuda_check(cudaMemcpyAsync(&h_unserved[c], d_unserved, 4, cudaMemcpyDeviceToHost, st), "D2H(unserved)");
         }
         if (pipeline_trace()) ch.tr.mark(2, st);
@@ -2310,7 +2367,9 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
         if (!cc.issued) return;
         cuda_check(cudaEventSynchronize(cc.kernels), "sync(kernels)");
         const uint64_t ntok = want_tokens ? s.h_totals[4] : 0;
+        const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
         if (want_tags && tok_total + ntok > token_capacity) { overflow = true; cc.issued = false; }
+        if (score_total + nsc > score_capacity) overflow = true;
         cudaStream_t so = s.stream_out;
         cuda_check(cudaStreamWaitEvent(so, cc.kernels, 0), "cudaStreamWaitEvent");
         if (!overflow) {
@@ -2333,11 +2392,14 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
                 cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.d_tok, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
                 if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.d_cand, ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
             }
+            if (nsc)
+                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
         }
         cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
         if (pipeline_trace()) ch.tr.mark(3, so);
         cc.copied = !overflow && cc.nb != 0;
         tok_total += ntok;
+        score_total += nsc;
     };
     // A runs kDepth - 2 chunks ahead of B, B one chunk ahead of C (a scratch is free again when its chunk's C is done)
     constexpr size_t kAheadA = kDepth - 2;
@@ -2360,7 +2422,11 @@ int vpt_predict_batch_compact(const vpt_predictor* p, const uint8_t* utf8, const
     if (n_boundaries_out) *n_boundaries_out = nb_total;
     if (n_tokens_total_out) *n_tokens_total_out = tok_total;
     if (n_unserved_out) *n_unserved_out = unserved_total;
-    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: bits_capacity_words/token_capacity: too small for the batch");
+    if (n_scores_total_out) *n_scores_total_out = score_total;
+    if (overflow) {
+        if (score_total > score_capacity) throw Error(kInvalidArgument, "InvalidArgumentError: score_capacity: too small for the batch");
+        throw Error(kInvalidArgument, "InvalidArgumentError: bits_capacity_words/token_capacity: too small for the batch");
+    }
     return kOk;
     VPT_API_END
 }
@@ -2395,11 +2461,26 @@ std::vector<std::pair<size_t, size_t>> span_chunks(const uint64_t* byte_offsets,
 int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_docs, int no_norm,
                     uint32_t wsconst_types, uint32_t* n_tokens_out, uint8_t* status_out, uint32_t* token_ends_out,
                     int32_t* token_ids_out, uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_tokens_total_out) {
+    return vpt_token_spans_tag_scores(p, utf8, byte_offsets, n_docs, no_norm, wsconst_types, n_tokens_out, status_out,
+                                      token_ends_out, token_ids_out, token_cands_out, token_capacity, n_tokens_total_out,
+                                      nullptr, 0, nullptr);
+}
+
+int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_docs,
+                               int no_norm, uint32_t wsconst_types, uint32_t* n_tokens_out, uint8_t* status_out,
+                               uint32_t* token_ends_out, int32_t* token_ids_out, uint8_t* token_cands_out,
+                               size_t token_capacity, uint64_t* n_tokens_total_out, int32_t* tag_scores_out,
+                               size_t score_capacity, uint64_t* n_scores_total_out) {
     VPT_API_BEGIN
     if (n_tokens_total_out) *n_tokens_total_out = 0;
+    if (n_scores_total_out) *n_scores_total_out = 0;
     const bool want_tags = token_ids_out != nullptr || token_cands_out != nullptr;
+    if (tag_scores_out && !want_tags)
+        throw Error(kInvalidArgument, "InvalidArgumentError: tag_scores_out: needs token_ids_out (tag prediction)");
     const bool tags = check_lines_flags(p, wsconst_types, want_tags);  // false with n_tags == 0: every token id is -1
     const size_t nt = tags ? p->n_tags : 0;
+    const bool want_scores = tags && tag_scores_out != nullptr;  // (a model without tag slots has no scores)
+    const size_t score_len = want_scores ? device_score_len_bound(p) : 0;
     if (want_tags && (!token_ids_out || (nt && !token_cands_out)))
         throw Error(kInvalidArgument, "InvalidArgumentError: token_ids_out/token_cands_out: must not be NULL");
     if (!byte_offsets || !n_tokens_out || !status_out)
@@ -2443,7 +2524,7 @@ int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t*
         ch.byte_lo = byte_offsets[ch.s_lo];
         ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
     }
-    uint64_t tok_total = 0;
+    uint64_t tok_total = 0, score_total = 0;
     bool overflow = false;
 
     auto stage_b = [&](size_t c) {
@@ -2529,7 +2610,12 @@ int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t*
             ta.tok_work = static_cast<uint32_t*>(s.d_tokwork);
             ta.text_base = 0;
             ta.norm = normalize ? 1 : 0;
-            cuda_check(launch_tags(p->dt, ta, st), "launch(tags)");
+            if (want_scores) {
+                const TagScoreArgs sc = bind_tag_scores(s, nc, score_len);
+                cuda_check(launch_tags(p->dt, ta, st, &sc), "launch(tags)");
+            } else {
+                cuda_check(launch_tags(p->dt, ta, st), "launch(tags)");
+            }
         }
         Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
         g.token_ends = static_cast<uint32_t*>(s.d_ends);
@@ -2545,7 +2631,9 @@ int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t*
         if (!cc.issued) return;
         cuda_check(cudaEventSynchronize(cc.kernels), "sync(kernels)");
         const uint64_t ntok = s.h_totals[4];
+        const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
         if (tok_total + ntok > token_capacity || (ntok && !token_ends_out)) overflow = true;
+        if (score_total + nsc > score_capacity) overflow = true;
         cudaStream_t so = s.stream_out;
         cuda_check(cudaStreamWaitEvent(so, cc.kernels, 0), "cudaStreamWaitEvent");
         if (!overflow) {
@@ -2558,10 +2646,13 @@ int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t*
                     if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.d_cand, ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
                 }
             }
+            if (nsc)
+                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
         }
         cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
         if (pipeline_trace()) ch.tr.mark(3, so);
         tok_total += ntok;
+        score_total += nsc;
     };
     // A runs kDepth - 2 chunks ahead of B, B one chunk ahead of C (a scratch is free again when its chunk's C is done)
     constexpr size_t kAheadA = kDepth - 2;
@@ -2579,7 +2670,11 @@ int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t*
     if (pipeline_trace())
         for (size_t c = 0; c < nchunks; ++c) chunks[c].cs.tr.print("spans", c, chunks[c].cs.n, chunks[0].cs.tr);
     if (n_tokens_total_out) *n_tokens_total_out = tok_total;
-    if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: token_capacity: too small for the batch");
+    if (n_scores_total_out) *n_scores_total_out = score_total;
+    if (overflow) {
+        if (score_total > score_capacity) throw Error(kInvalidArgument, "InvalidArgumentError: score_capacity: too small for the batch");
+        throw Error(kInvalidArgument, "InvalidArgumentError: token_capacity: too small for the batch");
+    }
     if (want_tags && !tags) std::fill(token_ids_out, token_ids_out + tok_total, -1);  // a model without tag slots
     return kOk;
     VPT_API_END

@@ -123,9 +123,13 @@ __global__ void __launch_bounds__(kTagWarps * 32, kLocateOnly ? 8 : 1) k_tags(De
 //                 to a work list (one atomic per warp)
 //   k_tok_score   the listed tokens, dense lanes: bias + tag weights + arg-max
 // Both are grid-stride loops over a resident grid (the token count is known on the device only).
+// kScores (TagScoreArgs, tags.hpp): the lookup also writes every record's score count, k_score_block / k_score_scan turn
+// the counts into offsets, and k_tok_score stores each listed token's score vector at its record's offset.  Without it
+// the kernels are the ones of the path without scores.
 constexpr int kTokTagThreads = 128;
 constexpr int kTokWorkHead = 4;  // words in front of the work list: [0] = entries
-__global__ void __launch_bounds__(kTokTagThreads) k_tok_lookup(DevTags t, TagArgs a) {
+template <bool kScores>
+__global__ void __launch_bounds__(kTokTagThreads) k_tok_lookup(DevTags t, TagArgs a, TagScoreArgs sc) {
     const uint64_t ntok = a.tok_base[a.n_sent];
     const uint32_t nt = t.n_tags;
     const int lane = threadIdx.x & 31;
@@ -149,6 +153,7 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_lookup(DevTags t, TagArg
             a.tok_ids[rec] = tok;
             if (!listed)
                 for (uint32_t k = 0; k < nt; ++k) a.tok_cands[rec * nt + k] = uint8_t(255);
+            if (kScores) sc.rec_off[rec] = listed ? tag_score_count(t.tok_info[tid], nt) : 0u;
         }
         const unsigned m = __ballot_sync(kFull, listed);
         if (m) {
@@ -160,7 +165,8 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_lookup(DevTags t, TagArg
     }
 }
 
-__global__ void __launch_bounds__(kTokTagThreads) k_tok_score(DevTags t, TagArgs a) {
+template <bool kScores>
+__global__ void __launch_bounds__(kTokTagThreads) k_tok_score(DevTags t, TagArgs a, TagScoreArgs sc) {
     const uint32_t nw = a.tok_work[0];
     const uint32_t nt = t.n_tags;
     for (uint32_t w = blockIdx.x * kTokTagThreads + threadIdx.x; w < nw; w += gridDim.x * kTokTagThreads) {
@@ -170,10 +176,70 @@ __global__ void __launch_bounds__(kTokTagThreads) k_tok_score(DevTags t, TagArgs
 #pragma unroll
         for (int k = 0; k < kTagMaxSlots; ++k) cand[k] = -1;
         // (characters [d.z, d.z + n_after) are the token's last character and what follows it in its sentence)
-        const int32_t tok = tag_score_token(t, uint32_t(a.tok_ids[rec]), a.char_states ? a.char_states + d.z : nullptr,
-                                            a.type_states ? a.type_states + d.z : nullptr, 0, d.y >> 16, cand, a.n_unserved);
+        int32_t* out = nullptr;
+        if (kScores) out = sc.scores + sc.blk[rec / kScoreScanBlock] + sc.rec_off[rec];
+        const int32_t tok = tag_score_token<kScores>(t, uint32_t(a.tok_ids[rec]), a.char_states ? a.char_states + d.z : nullptr,
+                                                     a.type_states ? a.type_states + d.z : nullptr, 0, d.y >> 16, cand,
+                                                     a.n_unserved, out);
         if (tok < 0) a.tok_ids[rec] = -1;
         for (uint32_t k = 0; k < nt; ++k) a.tok_cands[uint64_t(rec) * nt + k] = (tok >= 0 && cand[k] >= 0) ? uint8_t(cand[k]) : uint8_t(255);
+    }
+}
+
+// Offsets of the score vectors, step 1: exclusive prefix of the records' score counts inside each block of
+// kScoreScanBlock records (grid over max_tokens: the record count is known on the device only) and the block's total.
+__global__ void __launch_bounds__(kScoreScanBlock) k_score_block(TagArgs a, TagScoreArgs sc) {
+    __shared__ uint32_t s_w[kScoreScanBlock / 32];
+    const uint64_t ntok = a.tok_base[a.n_sent];
+    const uint64_t rec = uint64_t(blockIdx.x) * kScoreScanBlock + threadIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (uint64_t(blockIdx.x) * kScoreScanBlock >= ntok) {
+        if (threadIdx.x == 0) sc.blk[blockIdx.x] = 0;
+        return;
+    }
+    const uint32_t v = rec < ntok ? sc.rec_off[rec] : 0u;
+    const uint32_t incl = warp_incl_scan(v, lane);
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    uint32_t base = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < kScoreScanBlock / 32; ++w) {
+        if (w < warp) base += s_w[w];
+        tot += s_w[w];
+    }
+    if (rec < ntok) sc.rec_off[rec] = base + incl - v;
+    if (threadIdx.x == 0) sc.blk[blockIdx.x] = tot;
+}
+
+// step 2: exclusive prefix of the block totals (one block, 1024 totals per round); the chunk's total behind them and in
+// the pinned host word
+__global__ void __launch_bounds__(1024) k_score_scan(TagScoreArgs sc, uint64_t nblk) {
+    __shared__ uint64_t s_w[32];
+    __shared__ uint64_t s_carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    for (uint64_t lo = 0; lo < nblk; lo += 1024) {
+        const uint64_t i = lo + threadIdx.x;
+        const uint64_t v = i < nblk ? sc.blk[i] : 0;
+        uint64_t incl = v;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint64_t o = __shfl_up_sync(kFull, incl, d);
+            if (lane >= d) incl += o;
+        }
+        if (lane == 31) s_w[warp] = incl;
+        __syncthreads();
+        uint64_t base = s_carry;
+        for (int w = 0; w < warp; ++w) base += s_w[w];
+        if (i < nblk) sc.blk[i] = base + incl - v;
+        __syncthreads();
+        if (threadIdx.x == 1023) s_carry = base + incl;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        sc.blk[nblk] = s_carry;
+        if (sc.total_host) *sc.total_host = s_carry;
     }
 }
 
@@ -323,8 +389,9 @@ cudaError_t launch_rule_lookup(const DevTagRules& r, const TagArgs& a, int32_t* 
     return cudaGetLastError();
 }
 
-cudaError_t launch_tags(const DevTags& t, const TagArgs& a, cudaStream_t stream) {
+cudaError_t launch_tags(const DevTags& t, const TagArgs& a, cudaStream_t stream, const TagScoreArgs* scores) {
     if (a.n_sent == 0) return cudaSuccess;
+    if (scores && (!a.tok_desc || !a.tok_base || !scores->rec_off || !scores->blk || !scores->scores)) return cudaErrorInvalidValue;
     const uint64_t nblocks = (a.n_sent + kTagWarps - 1) / kTagWarps;
     if (a.tok_desc && a.tok_base) k_tags<true><<<unsigned(nblocks), kTagWarps * 32, 0, stream>>>(t, a);
     else k_tags<false><<<unsigned(nblocks), kTagWarps * 32, 0, stream>>>(t, a);
@@ -344,8 +411,18 @@ cudaError_t launch_tags(const DevTags& t, const TagArgs& a, cudaStream_t stream)
         }
         const uint64_t want = (a.max_tokens + kTokTagThreads - 1) / kTokTagThreads;
         // (resident blocks per SM: 16 x 128 threads at 32 registers, 8 x 128 at 56)
-        k_tok_lookup<<<unsigned(std::min<uint64_t>(want, uint64_t(sm_count[dev]) * 16)), kTokTagThreads, 0, stream>>>(t, a);
-        k_tok_score<<<unsigned(std::min<uint64_t>(want, uint64_t(sm_count[dev]) * 8)), kTokTagThreads, 0, stream>>>(t, a);
+        const unsigned lookup_grid = unsigned(std::min<uint64_t>(want, uint64_t(sm_count[dev]) * 16));
+        const unsigned score_grid = unsigned(std::min<uint64_t>(want, uint64_t(sm_count[dev]) * 8));
+        if (scores) {
+            const uint64_t nblk = (a.max_tokens + kScoreScanBlock - 1) / kScoreScanBlock;
+            k_tok_lookup<true><<<lookup_grid, kTokTagThreads, 0, stream>>>(t, a, *scores);
+            k_score_block<<<unsigned(nblk), kScoreScanBlock, 0, stream>>>(a, *scores);
+            k_score_scan<<<1, 1024, 0, stream>>>(*scores, nblk);
+            k_tok_score<true><<<score_grid, kTokTagThreads, 0, stream>>>(t, a, *scores);
+        } else {
+            k_tok_lookup<false><<<lookup_grid, kTokTagThreads, 0, stream>>>(t, a, TagScoreArgs{});
+            k_tok_score<false><<<score_grid, kTokTagThreads, 0, stream>>>(t, a, TagScoreArgs{});
+        }
     }
     return cudaGetLastError();
 }

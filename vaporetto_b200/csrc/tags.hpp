@@ -180,6 +180,19 @@ VPT_TAG_HD uint64_t tag_hash_finish(uint64_t h) {
 }
 constexpr uint64_t kTagHashInit = 0xCBF29CE484222325ull;
 
-cudaError_t launch_tags(const DevTags& t, const TagArgs& a, cudaStream_t stream);
+// Tag candidate scores of the per-token path (vpt_predict_batch_compact_tag_scores, vpt_token_spans_tag_scores): record r
+// with token id >= 0 gets its token's whole score vector (tag_score_count entries), the vectors of the chunk concatenated
+// in record order.  k_tok_lookup writes each record's count, a block scan + a one-block scan of the block totals turn
+// the counts into offsets, k_tok_score stores the vectors there.
+constexpr int kScoreScanBlock = 1024;   // records per block of the offset scan
+struct TagScoreArgs {
+    uint32_t* rec_off = nullptr;        // [max_tokens] scratch: score count of the record, then its offset inside its block
+    uint64_t* blk = nullptr;            // [max_tokens / kScoreScanBlock + 2] scratch: block totals, then their prefix
+    int32_t* scores = nullptr;          // [max_tokens x the longest vector] out: the chunk's score vectors
+    uint64_t* total_host = nullptr;     // pinned host word that receives the number of scores of the chunk
+};
+
+// scores: nullable; with it (and the per-token path: tok_desc) the score vectors come out as well
+cudaError_t launch_tags(const DevTags& t, const TagArgs& a, cudaStream_t stream, const TagScoreArgs* scores = nullptr);
 
 }  // namespace vpt

@@ -136,14 +136,31 @@ VPT_HD void add_scorer(const TagKey* __restrict__ keys, const uint8_t* cnt, uint
     }
 }
 
+// Number of scores a token of the table gets: its whole score vector (bias_len entries), or 0 when its slots' candidates
+// overrun the vector -- exactly the tokens tag_score_token answers -1 for after the `usable` check.  k_tok_lookup sizes
+// the score output with it before k_tok_score computes the scores.
+VPT_HD uint32_t tag_score_count(const TagTokenInfo& ti, uint32_t nt) {
+    uint32_t off = 0;
+    for (uint32_t k = 0; k < ti.n_slots && k < nt; ++k) {
+        const uint32_t nc = ti.cand[k];
+        if (nc >= 2) {
+            if (off + nc > ti.bias_len) return 0;
+            off += nc;
+        }
+    }
+    return ti.bias_len;
+}
+
 // Tag prediction of one token (bytes [bytes, bytes + len) of the text; `i` = index of its last character inside the
 // sentence's `n` characters whose pattern-id states start at cst / tst): token lookup, bias + tag weights of both scorers,
 // first strict maximum per tag slot (TagPredictor::predict, predictor.rs:286-304).  Returns the token id or -1 and the
-// chosen candidates in cand[].
+// chosen candidates in cand[].  kStoreScores: a token answered with its id also gets its whole score vector (the
+// `scores` Predictor::predict_tags keeps with store_tag_scores, tag_score_count(ti) entries) in scores_out[].
 // (the part behind the token lookup: `tid` is a token of the table)
+template <bool kStoreScores = false>
 VPT_HD int32_t tag_score_token(const DevTags& t, uint32_t tid, const uint32_t* __restrict__ cst,
                                                    const uint32_t* __restrict__ tst, uint32_t i, uint32_t n, int32_t* cand,
-                                                   uint32_t* n_unserved) {
+                                                   uint32_t* n_unserved, int32_t* __restrict__ scores_out = nullptr) {
     TagTokenInfo ti;
     {
         const uint4* q = reinterpret_cast<const uint4*>(t.tok_info + tid);
@@ -184,6 +201,8 @@ VPT_HD int32_t tag_score_token(const DevTags& t, uint32_t tid, const uint32_t* _
             cand[k] = nc == 1 ? 0 : -1;
         }
     }
+    if (kStoreScores)
+        for (uint32_t k = 0; k < ns; ++k) scores_out[k] = scores[k];
     return int32_t(tid);
 }
 
