@@ -496,7 +496,9 @@ int vpt_tag_rules_new(const vpt_predictor* predictor, uint64_t n_rules, const ui
                       const uint8_t* tags, uint64_t tags_len, vpt_tag_rules** out);
 void vpt_tag_rules_free(vpt_tag_rules* rules);
 /* The largest device output buffer, in bytes, that a chunk of a call with these rules has used (a diagnostic of the
- * output sizing: a chunk's buffer is sized by the rule suffixes its tokens actually matched, not by the longest rule). */
+ * output sizing: a chunk's buffer is sized by the rule suffixes its tokens actually matched, not by the longest rule).
+ * On a stream with score dumps (vpt_line_stream_new_scores) it is the buffer of the token lines, which the rules size;
+ * the dumps behind them are sized separately. */
 uint64_t vpt_tag_rules_max_output(const vpt_tag_rules* rules);
 
 /* vpt_tokenize_lines_tags with `rules` (nullable: NULL is vpt_tokenize_lines_tags).  Same arguments and errors; a rule's
@@ -509,6 +511,34 @@ int vpt_tokenize_lines_tags_rules(const vpt_predictor* predictor, const vpt_tag_
 int vpt_line_stream_new_rules(const vpt_predictor* predictor, const vpt_tag_rules* rules, int kind, int no_norm,
                               uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
                               vpt_line_stream** out);
+
+/* ---- Score dumps: the predict CLI's --scores and --tag-scores (predict/src/main.rs:66-93, 125-181) ------------------
+ *
+ * A VPT_STREAM_TOKENIZE line stream (with `rules`, nullable, as vpt_line_stream_new_rules) whose output is, per input
+ * line, the token line followed by the dumps the reference CLI prints for it:
+ *   VPT_DUMP_SCORES      valid lines: "{i}:{c_i}{c_i+1} {score_i}\n" per boundary, then "\n".  The characters are those
+ *                        of the predicted sentence (the KyteaFullwidthFilter image unless no_norm), the scores are
+ *                        predict's, before the wsconst filters, as i32 (sums wrap).  With no_norm the block comes
+ *                        before the line's '\n', as the CLI writes it (main.rs:136-141); otherwise after it.
+ *   VPT_DUMP_TAG_SCORES  every line: per token of the predicted sentence its surface (not escaped), then per tag slot of
+ *                        its tag model "\t" and the slot's "tag:score" pairs joined by ',' (one candidate: "tag:0"),
+ *                        then "\n"; one more "\n" after the last token.  Tag rules change the token line only.
+ * The output has no useful bound from the input (about 5x it with VPT_DUMP_SCORES), so there is no whole-buffer call.
+ * Device memory: with VPT_DUMP_TAG_SCORES each of the four chunks in flight also holds 4 x VPT_CHUNK_BYTES x the
+ * predictor's longest tag score vector bytes (512 MiB for 16 MiB chunks and 8-score vectors); see DESIGN §17.
+ * dumps == 0 is vpt_line_stream_new_rules.  Errors: those of vpt_line_stream_new_rules, and InvalidArgument for other
+ * `dumps` bits and for VPT_DUMP_TAG_SCORES without predict_tags or with a model without tag slots.
+ * Deviations from the reference, each where it panics or prints stale data:
+ *   1. A rejected line (empty, NUL, invalid UTF-8) gives the tag block " \n\n"; the reference prints the token " " with
+ *      the candidates of a stale entry of the last tagged line (sentence.rs:140-158, 1234), or panics if there is none.
+ *   2. VPT_DUMP_TAG_SCORES without tag prediction or tag slots is refused here; the reference panics at the first token.
+ *   3. A token whose slots list more candidates than its score vector has prints its surface alone; the reference
+ *      panics on scores[i]. */
+#define VPT_DUMP_SCORES 1u
+#define VPT_DUMP_TAG_SCORES 2u
+int vpt_line_stream_new_scores(const vpt_predictor* predictor, const vpt_tag_rules* rules, int no_norm,
+                               uint32_t wsconst_types, int predict_tags, uint32_t dumps, vpt_stream_write_fn write,
+                               void* ctx, vpt_line_stream** out);
 
 /* ---- Token spans: vaporetto_tantivy's token_stream for a batch of documents ---------------------------------------
  *

@@ -448,13 +448,21 @@ class LineStream {
 public:
     using Sink = std::function<void(const uint8_t* bytes, size_t n)>;
     /// kind: VPT_STREAM_TOKENIZE (`sink` receives the tokenised lines) or VPT_STREAM_EVALUATE (`sink` may be empty).
-    /// tag_rules: as in Predictor::tokenize_lines.
+    /// tag_rules: as in Predictor::tokenize_lines.  dumps: VPT_DUMP_SCORES | VPT_DUMP_TAG_SCORES, the predict CLI's
+    /// --scores / --tag-scores behind every token line (VPT_STREAM_TOKENIZE only; vpt_line_stream_new_scores).
     LineStream(const Predictor& predictor, int kind, Sink sink, bool no_norm = false, uint32_t wsconst_types = 0,
-               bool predict_tags = false, const TagRules* tag_rules = nullptr)
+               bool predict_tags = false, const TagRules* tag_rules = nullptr, uint32_t dumps = 0)
         : sink_(std::move(sink)) {
-        detail::check(vpt_line_stream_new_rules(predictor.handle(), detail::rules_handle(tag_rules), kind, no_norm ? 1 : 0,
-                                                wsconst_types, predict_tags ? 1 : 0, sink_ ? &LineStream::write : nullptr,
-                                                this, &h_));
+        if (dumps && kind != VPT_STREAM_TOKENIZE)
+            throw VaporettoError(VPT_INVALID_ARGUMENT, "InvalidArgumentError: dumps: VPT_STREAM_TOKENIZE only");
+        if (dumps)
+            detail::check(vpt_line_stream_new_scores(predictor.handle(), detail::rules_handle(tag_rules), no_norm ? 1 : 0,
+                                                     wsconst_types, predict_tags ? 1 : 0, dumps,
+                                                     sink_ ? &LineStream::write : nullptr, this, &h_));
+        else
+            detail::check(vpt_line_stream_new_rules(predictor.handle(), detail::rules_handle(tag_rules), kind, no_norm ? 1 : 0,
+                                                    wsconst_types, predict_tags ? 1 : 0, sink_ ? &LineStream::write : nullptr,
+                                                    this, &h_));
     }
     LineStream(const LineStream&) = delete;
     LineStream& operator=(const LineStream&) = delete;

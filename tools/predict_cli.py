@@ -3,17 +3,22 @@
 vpt_tokenize_lines fed in pieces): stdin lines -> space-separated tokens on stdout, everything between the two (line
 splitting, full-width pre-filter, scoring, --wsconst post-filters, output text) on the GPU.
 
-    python tools/predict_cli.py --model model.bin[.zst] [--no-norm] [--wsconst D] [--wsconst R] ... < in.txt > out.txt
+    python tools/predict_cli.py --model model.bin[.zst] [--no-norm] [--wsconst D] [--wsconst R] ... \
+        [--predict-tags] [--scores] [--tag-scores] < in.txt > out.txt
 
 Input of any size is read in pieces of up to 16 MiB, and the output is written as it comes: memory does not grow with the
 input.  When nothing more is waiting on stdin, the output of every complete line read so far is written and flushed, so
 an interactive session or a slow producer gets each line back as soon as it is entered, as with the reference.
 
-Options not on the device path (--scores, --tag-scores) are rejected; use the Sentence API
-(vaporetto_b200.Sentence / include/vaporetto_b200.hpp) for tags.  For the tag candidate scores --tag-scores prints, call
-the library: Predictor.predict_batch_compact(..., tags=True, tag_scores=True) or Predictor.token_spans(..., tags=True,
-tag_scores=True) and the result's tag_candidates(r) for a batch, Predictor.store_tag_scores(True) + Token.tag_candidates()
-for one sentence (C: vpt_predict_batch_compact_tag_scores, vpt_token_spans_tag_scores).
+--scores and --tag-scores print the reference's dumps behind each token line, written on the device as well
+(vpt_line_stream_new_scores): every boundary's characters and score, and every token's tag candidates with their scores.
+Three differences from the reference, where it panics or prints stale data: --tag-scores needs --predict-tags (the
+parser reports an error; the reference panics, as it does for a model without tag slots, which the library refuses); a
+rejected line (empty, NUL, invalid UTF-8) prints the tag block " " + two newlines, without the stale candidates the
+reference copies from an earlier line; a token whose tag slots list more candidates than its score vector holds prints
+its surface alone.  For tag candidate scores as data, call the library: Predictor.predict_batch_compact(...,
+tags=True, tag_scores=True) or Predictor.token_spans(..., tags=True, tag_scores=True) and the result's
+tag_candidates(r) for a batch, Predictor.store_tag_scores(True) + Token.tag_candidates() for one sentence.
 
 --tag-rules FILE is an extension: the reference CLI has no such option.  With --predict-tags it runs vaporetto_rules'
 PatternMatchTagger right after the tag prediction: every tag slot the model left empty for a token whose surface has
@@ -89,6 +94,8 @@ def main(argv=None) -> int:
     ap.add_argument("--wsconst", action="append", default=[], choices=list("DRHTKOG"),
                     help="Do not segment some character types: D Digit, R Roman, H Hiragana, T Katakana, K Kanji, O Other, G Grapheme cluster")
     ap.add_argument("--predict-tags", action="store_true", help="Predicts POS tags")
+    ap.add_argument("--scores", action="store_true", help="Prints boundary scores")
+    ap.add_argument("--tag-scores", action="store_true", help="Prints tag scores (needs --predict-tags)")
     ap.add_argument("--no-norm", action="store_true", help="Do not normalize input strings before prediction")
     ap.add_argument("--tag-rules", metavar="FILE",
                     help="Extension (not in the reference CLI): PatternMatchTagger rules, one `surface/tag1//tag3` per "
@@ -97,6 +104,8 @@ def main(argv=None) -> int:
     args = ap.parse_args(argv)
     if args.tag_rules and not args.predict_tags:
         ap.error("--tag-rules needs --predict-tags")
+    if args.tag_scores and not args.predict_tags:
+        ap.error("--tag-scores needs --predict-tags")
     rules = None
     if args.tag_rules:
         try:
@@ -112,7 +121,7 @@ def main(argv=None) -> int:
     inp, out = sys.stdin.buffer, sys.stdout.buffer
     t0 = time.perf_counter()
     with predictor.line_stream(no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
-                               tag_rules=tagger) as stream:
+                               tag_rules=tagger, scores=args.scores, tag_scores=args.tag_scores) as stream:
         while True:
             data = inp.read1(READ_BYTES)
             if not data:

@@ -132,6 +132,7 @@ ABI = [
     ("vpt_tokenize_lines_tags_rules", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, C.c_size_t,
                                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("vpt_line_stream_new_rules", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
+    ("vpt_line_stream_new_scores", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, C.c_uint32, _P, _P, C.POINTER(_P)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
     ("vpt_tag_n_slots", C.c_uint32, [_P, C.c_uint32]),
@@ -145,6 +146,7 @@ ABI = [
 # vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
 STREAM_WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
 STREAM_KINDS = {"tokenize": 0, "evaluate": 1}
+DUMP_SCORES, DUMP_TAG_SCORES = 1, 2  # VPT_DUMP_SCORES, VPT_DUMP_TAG_SCORES
 
 _lib = None
 
@@ -589,11 +591,14 @@ class Predictor:
         return r
 
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
-                    predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None) -> "LineStream":
+                    predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
+                    scores: bool = False, tag_scores: bool = False) -> "LineStream":
         """tokenize_lines (kind="tokenize") or evaluate_lines (kind="evaluate") on input fed in pieces of any size,
         with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream.  `tag_rules`
-        as in tokenize_lines."""
-        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules)
+        as in tokenize_lines.  `scores` / `tag_scores` (tokenize only; `tag_scores` needs predict_tags and a model with
+        tag slots) add the predict CLI's --scores / --tag-scores dumps behind every token line
+        (vpt_line_stream_new_scores)."""
+        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules, scores, tag_scores)
 
 
 class LineStream:
@@ -605,9 +610,12 @@ class LineStream:
     call close()."""
 
     def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool,
-                 tag_rules: Optional["PatternMatchTagger"] = None):
+                 tag_rules: Optional["PatternMatchTagger"] = None, scores: bool = False, tag_scores: bool = False):
         if kind not in STREAM_KINDS:
             raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize' or 'evaluate'")
+        dumps = (DUMP_SCORES if scores else 0) | (DUMP_TAG_SCORES if tag_scores else 0)
+        if dumps and kind != "tokenize":
+            raise VaporettoError(2, "InvalidArgumentError: scores, tag_scores: kind='tokenize' only")
         mask = _wsconst_mask(wsconst)
         self._predictor = predictor  # (the stream uses the predictor until it is closed)
         self._tag_rules = tag_rules  # (and the rules)
@@ -617,8 +625,12 @@ class LineStream:
         self._write = STREAM_WRITE_FN(self._sink)  # (kept alive as long as the stream)
         h = _P()
         rules = tag_rules._handle() if tag_rules is not None else None
-        _check(lib().vpt_line_stream_new_rules(predictor._h, rules, STREAM_KINDS[kind], int(no_norm), mask,
-                                               int(predict_tags), C.cast(self._write, _P), None, C.byref(h)))
+        if dumps:
+            _check(lib().vpt_line_stream_new_scores(predictor._h, rules, int(no_norm), mask, int(predict_tags), dumps,
+                                                    C.cast(self._write, _P), None, C.byref(h)))
+        else:
+            _check(lib().vpt_line_stream_new_rules(predictor._h, rules, STREAM_KINDS[kind], int(no_norm), mask,
+                                                   int(predict_tags), C.cast(self._write, _P), None, C.byref(h)))
         self._h = h
 
     def _sink(self, ctx, data, n):

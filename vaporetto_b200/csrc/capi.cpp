@@ -19,6 +19,7 @@
 #include "builder.hpp"
 #include "common.hpp"
 #include "device_model.hpp"
+#include "dump.hpp"
 #include "kernel_plan.hpp"
 #include "line_feed.hpp"
 #include "model.hpp"
@@ -79,6 +80,9 @@ struct Scratch {
     void* d_scoff = nullptr; size_t scoff_cap = 0; // tag candidate scores (TagScoreArgs): per-record counts / offsets,
     void* d_scblk = nullptr; size_t scblk_cap = 0; // block totals / prefix,
     void* d_tagsc = nullptr; size_t tagsc_cap = 0; // the chunk's score vectors
+    // score dumps of the lines path (dump.hpp): the token lines in front of their dumps, the per-line sizes
+    void* d_stage = nullptr; size_t stage_cap = 0;
+    void* d_dsize = nullptr; size_t dsize_cap = 0;
     // gold corpus and metrics (vpt_evaluate_lines)
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
@@ -89,15 +93,16 @@ struct Scratch {
     void* d_lc = nullptr; size_t lc_cap = 0;
     void* d_evtot = nullptr; size_t evtot_cap = 0;
     uint64_t* h_eval = nullptr;    // pinned, kEvalTotals + 1 x u64: a chunk's totals and error key
-    uint64_t* h_totals = nullptr;  // pinned, 8 x u64: boundaries, chars, lines, output bytes, tokens, first bit word, rule
-                                   // suffix bytes, tag scores
+    uint64_t* h_totals = nullptr;  // pinned, 10 x u64: boundaries, chars, lines, output bytes, tokens (score dumps: the
+                                   // writer's token line bytes), first bit word, rule suffix bytes, tag scores, then the
+                                   // score dumps' dump bytes and token line bytes
     uint32_t* h_side = nullptr; size_t side_cap = 0;  // pinned: first bit word of every chunk (vpt_predict_batch_compact)
     uint8_t* h_io = nullptr;       // pinned staging of the single-sentence call (vpt_predict), kSingleIoBytes
     void* d_io = nullptr;          // its device twin
     ~Scratch() {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
                         d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends, d_trule,
-                        d_scoff, d_scblk, d_tagsc,
+                        d_scoff, d_scblk, d_tagsc, d_stage, d_dsize,
                         d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
@@ -340,7 +345,7 @@ struct ScratchLease {
             cuda_check(cudaStreamCreateWithFlags(&s->stream_out, cudaStreamNonBlocking), "cudaStreamCreate");
             cuda_check(cudaEventCreateWithFlags(&s->ev_kernels, cudaEventDisableTiming), "cudaEventCreate");
             cuda_check(cudaEventCreateWithFlags(&s->ev_out, cudaEventDisableTiming), "cudaEventCreate");
-            cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s->h_totals), 64), "cudaMallocHost");
+            cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s->h_totals), 80), "cudaMallocHost");
         }
     }
     ~ScratchLease() {
@@ -1011,6 +1016,7 @@ struct LineJob {
     bool tags;         // tags predicted on the device
     int tag_mode;      // evaluate: how the system's tags compare with the gold's (kTags*)
     const vpt_tag_rules* rules = nullptr;  // PatternMatchTagger after fill_tags (tokenize with tags and rules only)
+    uint32_t dumps = 0;    // tokenize: the predict CLI's --scores / --tag-scores (kDumpScores | kDumpTagScores, dump.hpp)
 };
 
 // stage 0 of a chunk: H2D of its `nbytes` at `bytes`, newline counts, the number of lines to pinned host memory
@@ -1035,12 +1041,16 @@ void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* bytes) {
     cuda_check(cudaEventRecord(ch.split, st), "cudaEventRecord");
 }
 
+size_t device_score_len_bound(const vpt_predictor* p);
+TagScoreArgs bind_tag_scores(Scratch& s, uint64_t nc, size_t len_bound);
+
 // Scores the sentences of `a` (text, offsets, trims, n_sent set; `nbytes` bounds their bytes), runs the --wsconst
 // post-filters and, with `job.tags`, predicts the tags of every token into per-token records (the post-filters ran
 // first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
-// records; its output fields are left to the caller.
+// records; its output fields are left to the caller.  With the score dumps the boundary scores stay in `a.scores` and,
+// for --tag-scores, every record's score vector is stored through `sc`.
 TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job,
-                      TagRuleArgs* ra = nullptr) {
+                      TagRuleArgs* ra = nullptr, TagScoreArgs* sc = nullptr) {
     const bool normalize = job.normalize, tags = job.tags;
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
@@ -1056,7 +1066,7 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     a.scores = nullptr;
     DevModel dm = p.dm;
     dm.kytea_norm = normalize ? 1 : 0;
-    if (!scores_optional(dm)) {
+    if (!scores_optional(dm) || (job.dumps & kDumpScores)) {
         Scratch::ensure(s.d_scores, s.scores_cap, 4 * nbytes + 4);
         a.scores = static_cast<int32_t*>(s.d_scores);
     }
@@ -1128,7 +1138,8 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
         Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nbytes + 32);
         g.tok_work = static_cast<uint32_t*>(s.d_tokwork);
         g.norm = normalize ? 1 : 0;
-        cuda_check(launch_tags(p.dt, g, st), "launch(tags)");
+        if ((job.dumps & kDumpTagScores) && sc) *sc = bind_tag_scores(s, nbytes, device_score_len_bound(&p));
+        cuda_check(launch_tags(p.dt, g, st, (job.dumps & kDumpTagScores) && sc ? sc : nullptr), "launch(tags)");
         if (job.rules && ra) {
             // the rule id of every token, and the sum of the matched rules' suffix bounds in front of them
             Scratch::ensure(s.d_trule, s.trule_cap, 4 * nbytes + 16);
@@ -1171,6 +1182,66 @@ size_t split_lines(Scratch& s, LineChunk& ch) {
     return n;
 }
 
+// The score dumps of a chunk (dump.hpp) behind its token lines, which `t` wrote to the staging buffer: every line's dump
+// bytes and token line bytes with their prefixes and totals, one wait for the totals, then the output, sized exactly,
+// with its size in h_totals[3].  The token lines are placed by their computed sizes, not by their '\n's: a tag string
+// (of the model or of a rule) may hold a '\n'.
+void dump_stage(const vpt_predictor& p, Scratch& s, const TokArgs& t, const BatchArgs& a, const TagScoreArgs& sc,
+                const TagRuleArgs& ra, const LineJob& job) {
+    cudaStream_t st = s.stream;
+    const size_t n = size_t(t.n_sent);
+    DumpArgs d;
+    d.n_sent = n;
+    d.dumps = job.dumps;
+    d.norm = job.normalize ? 1 : 0;
+    d.text = t.text;
+    d.offsets = t.offsets;
+    d.trims = t.trims;
+    d.status = t.status;
+    d.n_chars = t.n_chars;
+    d.bound_offsets = t.bound_offsets;
+    d.boundaries = t.boundaries;
+    d.scores = a.scores;
+    if (t.tok_base) {
+        d.tok_base = t.tok_base;
+        d.tok_ids = t.tok_ids;
+        d.tok_cands = t.tok_cands;
+        d.n_tags = t.n_tags;
+        d.ts_slot = t.ts_slot;
+        d.ts_cand = t.ts_cand;
+        d.ts_ref = t.ts_ref;
+        d.ts_bytes = t.ts_bytes;
+        d.tok_rule = ra.tok_rule;
+        d.rules = ra.rules;
+    }
+    if (job.dumps & kDumpTagScores) {
+        d.tok_desc = static_cast<const uint4*>(s.d_tokdesc);
+        d.rec_off = sc.rec_off;
+        d.score_blk = sc.blk;
+        d.tag_scores = sc.scores;
+        d.tok_info = p.dt.tok_info;
+    }
+    const size_t nblk = (n + kDumpBlock - 1) / kDumpBlock;
+    Scratch::ensure(s.d_dsize, s.dsize_cap, 8 * (3 * n + 2 * nblk + 4));
+    d.size = static_cast<uint64_t*>(s.d_dsize);
+    d.tl_len = d.size + n;
+    d.tl_off = d.tl_len + n;
+    d.blk = d.tl_off + n;
+    d.total_host = &s.h_totals[8];
+    cuda_check(launch_dump_size(d, st), "launch(dump size)");
+    cuda_check(cudaStreamSynchronize(st), "sync(dump size)");
+    const uint64_t tok_bytes = s.h_totals[4], dump_bytes = s.h_totals[8];
+    // token_line_len restates the writers' sizes: a disagreement would misplace every later line of the chunk
+    if (s.h_totals[9] != tok_bytes)
+        throw Error(kInternal, "internal error: score dumps: token line sizes (" + std::to_string(s.h_totals[9]) +
+                                   ") disagree with the writer's (" + std::to_string(tok_bytes) + ")");
+    Scratch::ensure(s.d_out, s.out_cap, tok_bytes + dump_bytes + 4);
+    d.tok_lines = static_cast<const uint8_t*>(s.d_stage);
+    d.out = static_cast<uint8_t*>(s.d_out);
+    cuda_check(launch_dump_write(d, st), "launch(dump)");
+    s.h_totals[3] = tok_bytes - n + dump_bytes;  // dump_line writes each token line's '\n' itself
+}
+
 // stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
 void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
     cudaStream_t st = s.stream;
@@ -1178,32 +1249,37 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     s.h_totals[3] = 0;
     if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
     const size_t ng = (n + kGroup - 1) / kGroup;
+    // with the score dumps the token lines go to a staging buffer, and the dump writer puts them in front of their dumps
+    void*& tok_buf = job.dumps ? s.d_stage : s.d_out;
+    size_t& tok_cap = job.dumps ? s.stage_cap : s.out_cap;
     // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
     // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
     const size_t out_need = 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0);
-    Scratch::ensure(s.d_out, s.out_cap, out_need);
+    Scratch::ensure(tok_buf, tok_cap, out_need);
     BatchArgs a;
     a.text = ch.sp.text;
     a.offsets = ch.sp.offsets;
     a.trims = ch.sp.trims;
     a.n_sent = n;
     TagRuleArgs ra;
-    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job, &ra);
+    TagScoreArgs sc;
+    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job, &ra, &sc);
     if (ra.tok_rule) {
         // A rule's tag may be long on a short surface, so the rules' share of the output is sized from the suffixes the
         // chunk's tokens actually matched: the host waits for the rule lookup and reads their sum.
         cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
         cuda_check(cudaStreamSynchronize(st), "sync(rules)");
-        Scratch::ensure(s.d_out, s.out_cap, out_need + size_t(s.h_totals[6]));
+        Scratch::ensure(tok_buf, tok_cap, out_need + size_t(s.h_totals[6]));
         uint64_t seen = job.rules->max_out.load();
-        while (seen < s.out_cap && !job.rules->max_out.compare_exchange_weak(seen, s.out_cap)) {}
+        while (seen < tok_cap && !job.rules->max_out.compare_exchange_weak(seen, tok_cap)) {}
     }
     t.tok_state = static_cast<uint64_t*>(s.d_tokg);
     t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
     t.total = t.tok_state + ng + 1;
-    t.total_host = &s.h_totals[3];
-    t.out = static_cast<uint8_t*>(s.d_out);
+    t.total_host = &s.h_totals[job.dumps ? 4 : 3];
+    t.out = static_cast<uint8_t*>(tok_buf);
     cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
+    if (job.dumps) dump_stage(p, s, t, a, sc, ra, job);
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
 }
@@ -1804,6 +1880,29 @@ int vpt_line_stream_new_rules(const vpt_predictor* p, const vpt_tag_rules* rules
         throw Error(kInvalidArgument, "InvalidArgumentError: kind: VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE");
     const LineJob job = line_job(p, kind, no_norm, wsconst_types, predict_tags != 0, rules);
     if (kind == VPT_STREAM_TOKENIZE && !write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    *out = new vpt_line_stream(p, job, write, ctx);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_line_stream_new_scores(const vpt_predictor* p, const vpt_tag_rules* rules, int no_norm, uint32_t wsconst_types,
+                               int predict_tags, uint32_t dumps, vpt_stream_write_fn write, void* ctx,
+                               vpt_line_stream** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    LineJob job = line_job(p, VPT_STREAM_TOKENIZE, no_norm, wsconst_types, predict_tags != 0, rules);
+    if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
+    if (dumps & ~uint32_t(VPT_DUMP_SCORES | VPT_DUMP_TAG_SCORES))
+        throw Error(kInvalidArgument, "InvalidArgumentError: dumps: VPT_DUMP_SCORES and VPT_DUMP_TAG_SCORES only");
+    // Token::tag_candidates panics on a sentence without tag scores (sentence.rs:1230-1233): fill_tags did not run, or
+    // predicted nothing because the model has no tag slots (predictor.rs:553-555)
+    if ((dumps & VPT_DUMP_TAG_SCORES) && !predict_tags)
+        throw Error(kInvalidArgument, "InvalidArgumentError: dumps: VPT_DUMP_TAG_SCORES needs predict_tags");
+    if ((dumps & VPT_DUMP_TAG_SCORES) && !job.tags)
+        throw Error(kInvalidArgument, "InvalidArgumentError: dumps: VPT_DUMP_TAG_SCORES needs a model with tag slots");
+    job.dumps = dumps;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     *out = new vpt_line_stream(p, job, write, ctx);
     return kOk;
