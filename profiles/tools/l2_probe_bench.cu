@@ -4,6 +4,8 @@
 // build + run:
 //   mkdir -p build && nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/l2_probe_bench profiles/tools/l2_probe_bench.cu
 //   build/l2_probe_bench > build/l2_probe_bench.jsonl
+//   build/l2_probe_bench --probe-seq build/probe_slots.u32   (k_fused's own probe slots, from probe_slots.py: only
+//                                                             the `probe_seq` record_load test)
 // Output: one JSON object per line {"test": ..., "table_mb": ..., "ilp": ..., "gprobes_s": ..., "gbs": ...}.
 // The numbers give the peak of the scoring kernel's second roofline (bench.py: roofline_l1_lines).  "record_load" is
 // the test with load_record's own instructions and k_fused's geometry; the older "record32" kernels and the 32- and
@@ -11,6 +13,8 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
+#include <string>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -204,6 +208,52 @@ __global__ void __launch_bounds__(1024, 1) k_probe_mode(const char* table, uint3
     if (acc == 0x12345678u) *sink = acc + s_pad[0];
 }
 
+// As k_probe_mode<kL1a2, true> (load_record's form: allocating in L1, evict-last in L2), but the slots are k_fused's
+// own probe sequence on the config-2 text (profiles/tools/probe_slots.py) instead of uniformly random ones.  Probing
+// lane g takes entries g, g + P, g + 2P, ... (P probing lanes in the grid); the entry of the next round is loaded one
+// round ahead, without allocating in L1, so that only the records compete for the L1 the shared memory leaves.
+__global__ void __launch_bounds__(1024, 1) k_probe_seq(const char* table, const uint32_t* seq, uint32_t nseq, int iters,
+                                                        const uint4* sin, uint4* sout, size_t nvec, uint32_t* sink) {
+    extern __shared__ uint8_t s_pad[];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t acc = 0;
+    if ((warp & 3) == 3) {
+        const uint64_t pf = pol_first();
+        const size_t sw = size_t(blockIdx.x) * 8 + (warp >> 2), nsw = size_t(gridDim.x) * 8;
+        for (int i = 0; i < iters; ++i) {
+            const size_t k = ((size_t(i) * nsw + sw) * 32 + lane) % nvec;
+            uint32_t v[4];
+            asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(sin + k), "l"(pf));
+            __stcs(sout + k, make_uint4(v[0] + i, v[1], v[2], v[3]));
+        }
+        return;
+    }
+    const uint64_t pol = pol_last();
+    const uint64_t nprobe = uint64_t(gridDim.x) * 768;  // probing lanes in the grid
+    const uint64_t g = uint64_t(blockIdx.x) * 768 + (warp - (warp >> 2)) * 32 + lane;
+    auto next = [&](uint64_t e) {
+        uint32_t s;
+        asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(s) : "l"(seq + (e % nseq)));
+        return s;
+    };
+    uint32_t sl[2] = {next(g), next(g + nprobe)};
+    for (int i = 0; i < iters; ++i) {
+        const uint64_t e = (uint64_t(i + 1) * 2) * nprobe + g;
+        const uint32_t n0 = next(e), n1 = next(e + nprobe);
+        Rec32 r[2];
+#pragma unroll
+        for (int j = 0; j < 2; ++j) r[j] = load_mode<kL1a2>(table, sl[j], lane, pol);
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int w = 0; w < 8; ++w) acc += r[j].v[w] << w;
+        sl[0] = n0;
+        sl[1] = n1;
+    }
+    if (acc == 0x12345678u) *sink = acc + s_pad[0];
+}
+
 // random byte reads from a 37 KB shared-memory table (the perfect-hash seeds): LDS.U8 with random bank pattern
 __global__ void __launch_bounds__(1024) k_smem_seed(int iters, uint32_t* sink) {
     __shared__ uint8_t s_seed[37632];
@@ -256,7 +306,52 @@ static float time_ms(F&& launch, int reps) {
     return ms / reps;
 }
 
-int main() {
+// k_fused's probe sequence (probe_slots.py's output) at two shared-memory footprints, with the carve-out each needs:
+// the ratio of the rates is what the L1 the smaller footprint leaves is worth to the probes.
+static void probe_seq_test(const char* path, const char* table, uint32_t* sink, int n_sm) {
+    FILE* f = fopen(path, "rb");
+    if (!f) { fprintf(stderr, "%s: cannot open\n", path); exit(1); }
+    std::vector<uint32_t> h;
+    uint32_t buf[4096];
+    size_t got;
+    while ((got = fread(buf, 4, 4096, f)) > 0) h.insert(h.end(), buf, buf + got);
+    fclose(f);
+    uint32_t* seq;
+    CK(cudaMalloc(&seq, h.size() * 4));
+    CK(cudaMemcpy(seq, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
+    const size_t stream_bytes = size_t(64) << 20;
+    uint4 *sin, *sout;
+    CK(cudaMalloc(&sin, stream_bytes));
+    CK(cudaMalloc(&sout, stream_bytes));
+    CK(cudaMemset(sin, 0x11, stream_bytes));
+    int smem_sm = 0;
+    CK(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, 0));
+    const int iters = 256;
+    const double probes = double(n_sm) * 768 * iters * 2;
+    const int smem_kb[] = {217, 177};
+    for (int rep = 0; rep < 3; ++rep) {
+        for (int kb : smem_kb) {
+            const int smem = kb * 1024;
+            // the smallest carve-out that holds the CTA's shared memory and the 1 KB the system reserves per CTA
+            const int carve = std::min(100, ((smem + 1024) * 100 + smem_sm - 1) / smem_sm);
+            CK(cudaFuncSetAttribute(k_probe_seq, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            CK(cudaFuncSetAttribute(k_probe_seq, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
+            const float ms = time_ms([&] {
+                k_probe_seq<<<n_sm, 1024, smem>>>(table, seq, uint32_t(h.size()), iters, sin, sout, stream_bytes / 16, sink);
+            }, 20);
+            printf("{\"test\": \"record_load\", \"mode\": \"probe_seq\", \"smem_kb\": %d, \"carveout\": %d, \"probes\": %zu, "
+                   "\"ms\": %.4f, \"gprobes_s\": %.2f}\n",
+                   kb, carve, h.size(), ms, probes / ms / 1e6);
+            fflush(stdout);
+        }
+    }
+    CK(cudaGetLastError());
+    CK(cudaFree(seq));
+    CK(cudaFree(sin));
+    CK(cudaFree(sout));
+}
+
+int main(int argc, char** argv) {
     int dev = 0, n_sm = 0, clk_khz = 0;
     CK(cudaGetDevice(&dev));
     CK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -271,6 +366,12 @@ int main() {
     const int grid = n_sm * blocks_per_sm;
     const double nthreads = double(grid) * threads;
     printf("{\"test\": \"device\", \"sms\": %d, \"clock_mhz\": %.0f}\n", n_sm, clk_khz / 1000.0);
+    if (argc == 3 && std::string(argv[1]) == "--probe-seq") {
+        probe_seq_test(argv[2], static_cast<const char*>(table), sink, n_sm);
+        CK(cudaFree(table));
+        CK(cudaFree(sink));
+        return 0;
+    }
 
     {   // what the limit is made of: bytes per lane and lanes per line, L2-resident 23 MB table and an L1-sized 64 KB one
         const int iters = 64;

@@ -8,7 +8,10 @@
 //
 // One persistent CTA per SM = up to 4 independent 256-thread sub-blocks; a sub-block pulls 64-sentence groups from a
 // global ticket and, per group:
-//   stage   one TMA bulk copy (cp.async.bulk + mbarrier) of the group's UTF-8 bytes into shared memory
+//   load    every thread reads its 32-byte units of the group's UTF-8 bytes from global memory into registers
+//           (L1::no_allocate, evict-first in L2), where they stay until the scatter step: no shared-memory staging,
+//           so the shared memory is small enough for the 196 KB carve-out and the L1 it leaves (60 KB) holds the
+//           node records of frequent characters and pairs
 //   count   byte space, one thread per 32 bytes: SWAR masks of character starts, structural UTF-8 validation
 //           (continuation bytes == bytes the leads ask for), NUL; one block scan gives every thread the number of
 //           characters and sentence starts before its bytes -> group totals
@@ -42,7 +45,8 @@ namespace {
 constexpr int kFGroup = fused_detail::kGroupSentences;  // sentences per tile
 constexpr int kFSubThreads = 256;
 constexpr int kFWarps = kFSubThreads / 32;
-// Tile buffers: bytes of text staged per tile (multiple of 32) and character slots (characters + separators) per tile.
+// Tile buffers: bytes of text per tile (multiple of 32: a bound on the group's span, which the threads hold in registers)
+// and character slots (characters + separators) per tile.
 // 64 sentences of 40 characters need 7.4 KB and 2 760 slots; the buffers are sized so that 64 sentences of ragged
 // natural-length text (log-normal, mean 41 characters: 7.6 +- 0.6 KB, 2 840 +- 220 slots) still fit -- a group that does
 // not fit takes the slow path, and every later group waits in its look-back for the slow group's totals (with 8 192 B /
@@ -96,22 +100,26 @@ struct FLayout {
     static constexpr int kOffTypeB = kOffTypeA + (kCommon ? 4 * kFTypeSub : 0);
     static constexpr int kOffTyTab = kOffTypeB + (kCommon ? 4 * kFTypeSub : 0);
     static constexpr int kOffSub = kOffTyTab + kTypeTableBytes;
-    // per sub-block
-    static constexpr int kSText = 0;
-    static constexpr int kSRaw = kSText + kFTextCap + 32;
+    // per sub-block (the group's text is read into registers, not staged here)
+    static constexpr int kSRaw = 0;
     static constexpr int kSMeta = kSRaw + 4 * kFSlotAlloc;
     static constexpr int kSAcc = kSMeta + int(sizeof(MetaT)) * kFSlotAlloc;
     static constexpr int kSBitsS = kSAcc + (kOverflow ? 4 * kFSlotAlloc : 0);
     static constexpr int kSBitsX = kSBitsS + kFTextCap / 8 + 16;
     static constexpr int kSTab = kSBitsX + kFTextCap / 8 + 16;
-    static constexpr int kSBar = kSTab + ((int(sizeof(FTab)) + 15) & ~15);
-    static constexpr int kSubBytes = (kSBar + 16 + 127) & ~127;
-    static constexpr int kMaxSub = (227 * 1024 - kOffSub) / kSubBytes;
-    static constexpr int kSubBlocks = kMaxSub >= 4 ? 4 : kMaxSub;
+    static constexpr int kSubBytes = (kSTab + int(sizeof(FTab)) + 127) & ~127;
+    // four sub-blocks per SM (three with the overflow sums next to the seed table: kernel_plan.hpp)
+    static constexpr int kSubBlocks = plan_detail::fused_sub_blocks(kSeedsSmem, kOverflow);
     static constexpr int kThreads = kSubBlocks * kFSubThreads;
     static constexpr int kSmem = kOffSub + kSubBlocks * kSubBytes;
-    static_assert(kSubBlocks >= ((kOverflow && kSeedsSmem) ? 3 : 4),
-                  "shared memory budget: four sub-blocks per SM (three with the overflow sums next to the seed table)");
+    static_assert(kSmem <= 227 * 1024, "shared memory budget: more than a CTA may have");
+    // Shared memory and L1 are one 256 KB array per SM: the L1 is what the shared-memory carve-out leaves (H100
+    // carve-outs: ... 132, 164, 196, 228 KB), and it holds the node records of frequent characters and pairs.  With the
+    // 1 KB the system reserves per CTA, every variant fits the 196 KB carve-out (60 KB of L1 or more) except the two
+    // with overflow sums next to the seed table (three sub-blocks; 197 and 199 KB: the 228 KB carve-out).  The launch
+    // asks for the smallest carve-out that fits.
+    static constexpr int kCarveoutKB = (kOverflow && kSeedsSmem) ? 228 : 196;
+    static_assert(kSmem + 1024 <= kCarveoutKB * 1024, "shared memory exceeds the carve-out this variant is built for");
     static_assert(int(sizeof(Rings)) <= 4 * kFSlotAlloc, "fallback ring aliases the slot array");
     // what plan() reports (kernel_plan.hpp) is what this variant is built with
     static_assert(kFTextCap == plan_detail::fused_text_cap(kSeedsSmem, kStates, kOverflow), "text buffer differs from the plan");
@@ -197,11 +205,25 @@ __device__ __forceinline__ uint32_t type_of(uint32_t c, const uint8_t* s_tytab) 
     return type_from_table(s_tytab, c);
 }
 
-__device__ __forceinline__ uint32_t lds_window(const uint8_t* s_text, uint32_t pos) {
-    const uint32_t al = pos & ~3u;
-    const uint32_t lo = *reinterpret_cast<const uint32_t*>(s_text + al);
-    const uint32_t hi = *reinterpret_cast<const uint32_t*>(s_text + al + 4);
-    return __funnelshift_r(lo, hi, 8u * (pos & 3u));
+// The text goes from global memory straight into registers.  It is read once, so it is not allocated in L1 (which
+// holds the hot node records) and it is evict-first in L2 (which must keep the node table while the text and the
+// outputs stream through it).
+__device__ __forceinline__ uint4 ldg_text16(const uint8_t* p) {
+    uint4 v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_policy_evict_first()));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg_text4(const uint8_t* p) {
+    uint32_t v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(l2_policy_evict_first()));
+    return v;
+}
+
+// the bytes of word x whose bits are set in the 4-bit mask `keep` stay, the others read as spaces
+__device__ __forceinline__ uint32_t keep_bytes(uint32_t x, uint32_t keep) {
+    const uint32_t bm = ((keep * 0x00204081u) & 0x01010101u) * 0xFFu;  // bit j of `keep` -> byte j
+    return (x & bm) | (0x20202020u & ~bm);
 }
 
 // Exact validation + character count of one sentence by one warp, from global memory (slow path; the rules of
@@ -540,7 +562,6 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
     const int sub = threadIdx.x / kFSubThreads;
     const int tid = threadIdx.x % kFSubThreads, warp = tid >> 5, lane = tid & 31;
     uint8_t* sb = smem + Lay::kOffSub + sub * Lay::kSubBytes;
-    uint8_t* s_text = sb + Lay::kSText;
     uint32_t* s_raw_alloc = reinterpret_cast<uint32_t*>(sb + Lay::kSRaw);
     uint32_t* s_raw = s_raw_alloc + kFPadFront;
     MetaT* s_meta = reinterpret_cast<MetaT*>(sb + Lay::kSMeta) + kFPadFront;
@@ -548,7 +569,6 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
     uint32_t* s_sbits = reinterpret_cast<uint32_t*>(sb + Lay::kSBitsS);
     uint32_t* s_xbits = reinterpret_cast<uint32_t*>(sb + Lay::kSBitsX);
     FTab& T = *reinterpret_cast<FTab*>(sb + Lay::kSTab);
-    uint64_t* s_bar = reinterpret_cast<uint64_t*>(sb + Lay::kSBar);
     const uint8_t* __restrict__ text = a.text;
     uint64_t* const desc_b = a.group_bound;  // look-back descriptors (zeroed by the launcher, with the ticket)
     uint64_t* const desc_c = a.group_char;
@@ -567,14 +587,12 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
     }
     // character types by table: page table over c >> 8 + the sub-tables of the mixed pages (textnorm.hpp)
     for (int i = threadIdx.x; i < kTypeTableBytes; i += Lay::kThreads) s_tytab[i] = uint8_t(type_table_entry(uint32_t(i)));
-    if (tid == 0) mbar_init(s_bar, 1);
     __syncthreads();
 
     const uint64_t ngroups = (a.n_sent + kFGroup - 1) / kFGroup;
     // (the common shape separates sentences by two slots -- fused.cu checks it --: the separator loop of the scatter step,
     //  which a whole warp walks for the one lane that sees a sentence start, unrolls to two stores)
     const int gap = kCommon ? fused_detail::kCommonGap : cfg.gap;
-    uint32_t phase = 0;
 
     for (;;) {
         if (tid == 0) T.ticket = atomicAdd(a.ticket, 1u);
@@ -597,17 +615,49 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
 
         const uint64_t a0 = T.off[0] & ~15ull;
         const uint64_t end = T.off[ns];
+        // (the text cap is a bound on the group's span, rounded up to 16 bytes: the geometry plan() reports)
         bool fast = end >= T.off[0] && ((end - a0 + 15) & ~15ull) + 16 <= uint64_t(kFTextCap);
-        const uint32_t span = fast ? uint32_t((end - a0 + 15) & ~15ull) : 0u;
         const uint32_t lo_byte = uint32_t(T.off[0] - a0), hi_byte = fast ? uint32_t(end - a0) : 0u;
         int S = 0;
 
         if (fast) {
-            // ---- stage the group's bytes; meanwhile clear the slot stream and mark sentence starts / excluded bytes ----
-            if (tid == 0 && span) {
-                mbar_expect_tx(s_bar, span);
-                tma_bulk_g2s(s_text, text + a0, span, s_bar);
-            }
+            // ---- load the group's bytes; meanwhile clear the slot stream and mark sentence starts / excluded bytes ----
+            // Thread tid holds unit tid and unit 256 + tid (32 bytes each) in registers from the count step to the
+            // scatter step.  The bytes up to the next multiple of 16 behind the group's end are readable (the text buffer
+            // is padded to 16 bytes and an address has the alignment of its offset); bytes outside the group's
+            // [lo_byte, hi_byte) read as spaces (count step): never a continuation byte, never NUL.  The first word behind
+            // a unit (`halo`) comes from the next lane; the last lane of a warp loads its own.
+            auto load_unit = [&](uint32_t ub, uint32_t (&v)[8], uint32_t& h) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) v[i] = 0x20202020u;
+                h = 0x20202020u;
+                if (ub < hi_byte) {
+                    const uint4 q0 = ldg_text16(text + a0 + ub);
+                    v[0] = q0.x; v[1] = q0.y; v[2] = q0.z; v[3] = q0.w;
+                    if (ub + 16 < hi_byte) {
+                        const uint4 q1 = ldg_text16(text + a0 + ub + 16);
+                        v[4] = q1.x; v[5] = q1.y; v[6] = q1.z; v[7] = q1.w;
+                    }
+                    if (lane == 31 && ub + 32 < hi_byte) h = ldg_text4(text + a0 + ub + 32);
+                }
+            };
+            // bytes of the unit at ub that lie inside the group's range
+            auto range_mask = [&](uint32_t ub) {
+                uint32_t rm = 0xFFFFFFFFu;
+                if (ub < lo_byte) rm &= lo_byte - ub >= 32 ? 0u : 0xFFFFFFFFu << (lo_byte - ub);
+                if (ub + 32 > hi_byte) rm &= 0xFFFFFFFFu >> (ub + 32 - hi_byte);
+                return rm;
+            };
+            auto patch_unit = [&](uint32_t ub, uint32_t rm, uint32_t (&v)[8], uint32_t& h) {
+                if (rm != 0xFFFFFFFFu) {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) v[i] = keep_bytes(v[i], (rm >> (4 * i)) & 15u);
+                }
+                if (lane == 31 && ub + 32 < hi_byte && hi_byte - ub - 32 < 4) h = keep_bytes(h, (1u << (hi_byte - ub - 32)) - 1u);
+            };
+            uint32_t w[2][8], halo[2];
+#pragma unroll
+            for (int pass = 0; pass < 2; ++pass) load_unit(uint32_t(pass * kFSubThreads + tid) << 5, w[pass], halo[pass]);
             // (the separator slots of the slot stream are cleared by the scatter step itself; the front padding here)
             if (tid < kFPadFront) s_raw_alloc[tid] = 0;
             if (kOverflow)
@@ -633,19 +683,6 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                 }
             }
             fsub_sync(sub);
-            if (span) {
-                mbar_wait(s_bar, phase);
-                phase ^= 1;
-            }
-            // bytes of the staged span outside the group's range read as spaces: never a continuation byte, never NUL
-            if (tid < 64) {
-                const uint32_t pos = tid < 16 ? uint32_t(tid) : hi_byte + uint32_t(tid) - 16u;
-                if (tid < 16 ? pos < lo_byte : pos < span + 48u) s_text[pos] = 0x20;
-            }
-            // a sentence must not start on a continuation byte (with the structural check of the stream stage this
-            // makes every sentence valid on its own)
-            if (tid < ns && T.off[tid] < end && (s_text[uint32_t(T.off[tid] - a0)] & 0xC0u) == 0x80u) T.anomaly = 1;
-            fsub_sync(sub);
 
             // ---- count: one thread per 32-byte unit (two passes cover the tile buffer): character starts, NUL ------------
             // (whether the continuation bytes are where the lead bytes want them is checked by the stream stage, per
@@ -660,31 +697,30 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                 if (pass == 0 || nunits > kFSubThreads) {
                     if (u < nunits) {
                         const uint32_t ub = uint32_t(u) << 5;
-                        uint32_t w[8];
-                        {
-                            const uint4 q0 = *reinterpret_cast<const uint4*>(s_text + ub);
-                            const uint4 q1 = *reinterpret_cast<const uint4*>(s_text + ub + 16);
-                            w[0] = q0.x; w[1] = q0.y; w[2] = q0.z; w[3] = q0.w;
-                            w[4] = q1.x; w[5] = q1.y; w[6] = q1.z; w[7] = q1.w;
-                        }
+                        // bytes outside the group's range and excluded bytes (line terminators) are not characters
+                        const uint32_t rm = range_mask(ub);
+                        patch_unit(ub, rm, w[pass], halo[pass]);
                         uint32_t starts = 0, nul = 0;
 #pragma unroll
                         for (int i = 0; i < 8; ++i) {
-                            const uint32_t x = w[i];
+                            const uint32_t x = w[pass][i];
                             nul |= (x - 0x01010101u) & ~x;                           // bit 7 of a byte: the byte is zero
                             const uint32_t st80 = ~(x & ~(x << 1)) & 0x80808080u;    // not 10xxxxxx
                             starts |= ((((st80 >> 7) * 0x00204081u) >> 21) & 15u) << (4 * i);
                         }
                         if (nul & 0x80808080u) T.anomaly = 1;
-                        // bytes outside the group's range and excluded bytes (line terminators) are not characters
-                        uint32_t rm = 0xFFFFFFFFu;
-                        if (ub < lo_byte) rm &= lo_byte - ub >= 32 ? 0u : 0xFFFFFFFFu << (lo_byte - ub);
-                        if (ub + 32 > hi_byte) rm &= 0xFFFFFFFFu >> (ub + 32 - hi_byte);
                         const uint32_t ex = s_xbits[u], sbt = s_sbits[u] & rm;
+                        // a sentence must not start on a continuation byte (with the structural check of the stream
+                        // stage this makes every sentence valid on its own)
+                        if (sbt & ~starts) T.anomaly = 1;
                         starts &= rm & ~ex;
                         u_starts[pass] = starts;
                         u_sbits[pass] = sbt;
                         packed = __popc(starts) | (__popc(sbt) << 14) | (__popc(sbt & starts) << 22);
+                    }
+                    {
+                        const uint32_t next = __shfl_down_sync(kFull, w[pass][0], 1);
+                        if (lane != 31) halo[pass] = next;
                     }
                     // block scan of the packed counts
                     const uint32_t incl = warp_incl_scan(packed, lane);
@@ -724,20 +760,10 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                 for (int pass = 0; pass < 2; ++pass) {
                     const uint32_t mset = u_starts[pass] | u_sbits[pass];
                     if (mset == 0) continue;
-                    const uint32_t ub = uint32_t(pass * kFSubThreads + tid) << 5;
                     uint32_t G = u_excl[pass] & 0x3FFFu, K = (u_excl[pass] >> 14) & 0xFFu, NE = u_excl[pass] >> 22;
                     uint32_t slot = G + uint32_t(gap) * K;  // slot of the next character
                     uint32_t ol = G - NE + 1;               // its boundary index (valid once its sentence has started)
-                    // the unit's bytes travel in registers: a character's four-byte window is a funnel shift of two of
-                    // them (per-character loads from the text buffer would hit four banks: the lanes are 32 bytes apart)
-                    uint32_t w[9];
-                    {
-                        const uint4 q0 = *reinterpret_cast<const uint4*>(s_text + ub);
-                        const uint4 q1 = *reinterpret_cast<const uint4*>(s_text + ub + 16);
-                        w[0] = q0.x; w[1] = q0.y; w[2] = q0.z; w[3] = q0.w;
-                        w[4] = q1.x; w[5] = q1.y; w[6] = q1.z; w[7] = q1.w;
-                        w[8] = *reinterpret_cast<const uint32_t*>(s_text + ub + 32);
-                    }
+                    // a character's four-byte window is a funnel shift of two of the unit's registers
 #pragma unroll
                     for (int k = 0; k < 8; ++k) {
                         uint32_t nib = (mset >> (4 * k)) & 15u;
@@ -756,7 +782,7 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                                 if (is_start) { ++NE; --ol; }
                             }
                             if (is_start) {
-                                s_raw[slot] = __funnelshift_r(w[k], w[k + 1], 8 * jj);
+                                s_raw[slot] = __funnelshift_r(w[pass][k], k < 7 ? w[pass][k + 1] : halo[pass], 8 * jj);
                                 s_meta[slot] = kStates ? MetaT(ol | (G << 12)) : MetaT(ol);
                                 ++G; ++slot; ++ol;
                             }
@@ -901,13 +927,7 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                 k0 = k1;
                 continue;
             }
-            const uint64_t ra0 = T.off[k0] & ~15ull;
-            const uint32_t rspan = uint32_t((T.off[k1] - ra0 + 15) & ~15ull);
             const int Sr = gap + int(T.first[k1] - T.first[k0]) + gap * (k1 - k0);
-            if (tid == 0 && rspan) {
-                mbar_expect_tx(s_bar, rspan);
-                tma_bulk_g2s(s_text, text + ra0, rspan, s_bar);
-            }
             for (int i = tid; i < kFSlotAlloc / 4; i += kFSubThreads) reinterpret_cast<uint4*>(s_raw_alloc)[i] = make_uint4(0, 0, 0, 0);
             if (kOverflow)
                 for (int i = tid; i < kFSlotAlloc / 4; i += kFSubThreads) reinterpret_cast<uint4*>(s_acc - kFPadFront)[i] = make_uint4(0, 0, 0, 0);
@@ -915,25 +935,31 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
             if (kOverflow)
                 for (int i = tid; i < kFSlotAlloc; i += kFSubThreads) (s_meta - kFPadFront)[i] = MetaT(0);
             fsub_sync(sub);
-            if (rspan) {
-                mbar_wait(s_bar, phase);
-                phase ^= 1;
-            }
-            // scatter, one warp per sentence
+            // scatter, one warp per sentence, from global memory: a lane reads one word per 128-byte step and takes the
+            // word behind it from the next lane (the last lane reads its own)
             for (int k = k0 + warp; k < k1; k += kFWarps) {
                 const uint32_t n = T.first[k + 1] - T.first[k];
                 if (T.st[k] != 0) {
                     zero_sentence(a, T.obase + T.lb[k], T.cbase + T.first[k], n, lane);
                     continue;
                 }
-                const uint32_t rb0 = uint32_t(T.off[k] - ra0), rb1 = uint32_t(T.off[k + 1] - ra0) - T.trim[k];
+                const uint8_t* const st = text + (T.off[k] & ~3ull);  // offsets below are relative to it
+                const uint32_t rb0 = uint32_t(T.off[k] & 3u), rb1 = rb0 + uint32_t(T.off[k + 1] - T.off[k]) - T.trim[k];
                 uint32_t idx = uint32_t(gap) + (T.first[k] - T.first[k0]) + uint32_t(gap) * uint32_t(k - k0);
                 uint32_t ci = 0;  // characters of this sentence already placed
-                for (uint32_t wpos = rb0 & ~3u; wpos < rb1; wpos += 128) {
+                for (uint32_t wpos = 0; wpos < rb1; wpos += 128) {
                     const uint32_t addr = wpos + 4u * uint32_t(lane);
+                    uint32_t lo = 0, hi = 0;
+                    if (addr < rb1) {
+                        lo = ldg_text4(st + addr);
+                        if (lane == 31 && addr + 4 < rb1) hi = ldg_text4(st + addr + 4);
+                    }
+                    {
+                        const uint32_t next = __shfl_down_sync(kFull, lo, 1);
+                        if (lane != 31) hi = next;
+                    }
                     uint32_t smask = 0;
                     if (addr < rb1) {
-                        const uint32_t lo = *reinterpret_cast<const uint32_t*>(s_text + addr);
                         const uint32_t from = rb0 > addr ? rb0 - addr : 0u;
                         const uint32_t to = rb1 - addr < 4u ? rb1 - addr : 4u;
                         const uint32_t im80 = (from >= 4u ? 0u : 0x80808080u << (8 * from)) & (0x80808080u >> (8 * (4 - to)));
@@ -948,7 +974,7 @@ k_fused(DevModel m, BatchArgs a, StreamCfg cfg) {
                         if (smask & (1u << j)) {
                             const uint32_t gi = T.first[k] - T.first[k0] + ci + at;  // range-local character index
                             const uint32_t ol = T.lb[k] - T.lb[k0] + ci + at;        // range-local boundary index
-                            s_raw[idx + at] = lds_window(s_text, addr + uint32_t(j));
+                            s_raw[idx + at] = __funnelshift_r(lo, hi, 8u * uint32_t(j));
                             s_meta[idx + at] = kStates ? MetaT(ol | (gi << 12)) : MetaT(ol);
                             ++at;
                         }
@@ -988,7 +1014,17 @@ cudaError_t launch_fused_t(const DevModel& m, const BatchArgs& a, const StreamCf
     using Lay = FLayout<kSeeds, kCommon, kDeep, kStates>;
     static std::atomic<bool> attr_set[kMaxDevices] = {};  // (idempotent: set after the attribute call succeeded)
     if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(k_fused<kSeeds, kCommon, kDeep, kStates>, cudaFuncAttributeMaxDynamicSharedMemorySize, Lay::kSmem);
+        auto* k = k_fused<kSeeds, kCommon, kDeep, kStates>;
+        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Lay::kSmem);
+        if (e != cudaSuccess) return e;
+        // The smallest shared-memory carve-out that holds the CTA (with the 1 KB reserved per CTA), so that the rest of
+        // the SM's array is L1 for the node records.  The attribute is a percentage of the SM's shared memory, which the
+        // driver rounds up to the next carve-out it supports.
+        int smem_sm = 0;
+        e = cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+        if (e != cudaSuccess) return e;
+        const int carveout = std::min(100, int(((int64_t(Lay::kSmem) + 1024) * 100 + smem_sm - 1) / smem_sm));
+        e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
         if (e != cudaSuccess) return e;
         attr_set[dev] = true;
     }

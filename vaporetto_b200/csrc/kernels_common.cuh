@@ -26,10 +26,11 @@ struct Rec32 {
 
 // One 32-byte node record.  sm_90 has no 256-bit global load: the record is two 128-bit loads of the same 32-byte sector.
 // The loads allocate in L1.  Natural text is Zipf-like, so the nodes of frequent characters and character pairs are
-// probed again while they are still in the L1 that k_fused's shared memory leaves.  A config-2 step took 1.087 ms
-// against 1.442 ms with L1::no_allocate (H100 80GB HBM3, 700 W power limit; DESIGN §4).  The records are re-used from
-// L2, which on an H100 (50 MB) is smaller than the text and the outputs a batch streams through it, so they are loaded
-// with an evict-last policy and the text with an evict-first one (tma_bulk_g2s).
+// probed again while they are still in the L1 that k_fused's shared memory leaves (60 KB per SM in the 196 KB
+// carve-out; k_fused reads its text around L1).  A config-2 step took 1.087 ms against 1.442 ms with L1::no_allocate
+// when 28 KB of L1 were left (H100 80GB HBM3, 700 W power limit; DESIGN §4).  The records are re-used from L2, which
+// on an H100 (50 MB) is smaller than the text and the outputs a batch streams through it, so they are loaded with an
+// evict-last policy and the text with an evict-first one.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
     uint64_t pol;
     asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
