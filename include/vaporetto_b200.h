@@ -45,7 +45,8 @@ enum {
     VPT_SENT_OK = 0,
     VPT_SENT_EMPTY = 1,        /* "text: must contain at least one character" */
     VPT_SENT_NUL = 2,          /* "text: must not contain NULL" */
-    VPT_SENT_BAD_UTF8 = 3
+    VPT_SENT_BAD_UTF8 = 3,
+    VPT_SENT_BAD_RANGE = 4     /* vpt_token_spans_dev only: the document's offsets are not a range in the batch */
 };
 
 #define VPT_NO_PATTERN 0xFFFFFFFFu /* u32::MAX in char_pma_states / type_pma_states (boundary_tag_scorer.rs:122-123) */
@@ -592,6 +593,44 @@ int vpt_token_spans_tag_scores(const vpt_predictor* predictor, const uint8_t* ut
                                uint8_t* status_out, uint32_t* token_ends_out, int32_t* token_ids_out,
                                uint8_t* token_cands_out, size_t token_capacity, uint64_t* n_tokens_total_out,
                                int32_t* tag_scores_out, size_t score_capacity, uint64_t* n_scores_total_out);
+
+/* ---- Token spans of documents already in device memory ---------------------------------------------------------------
+ *
+ * vpt_token_spans over DEVICE buffers, for text that already lives on the GPU (cuDF / Arrow string columns: a chars buffer
+ * and int32 or int64 offsets; torch tensors).  The outputs are exactly those of vpt_token_spans for the same documents:
+ * the filter chain, statuses, token ends relative to the document and tag records; d_token_offsets is the exclusive prefix
+ * of the token counts, with the total behind it.
+ *
+ * Contract: the call never synchronises, allocates, creates events or streams, or writes host memory.  All its work is
+ * queued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream) and it may be captured in a CUDA graph.  Every
+ * output is sized by a bound the host knows (tokens <= characters <= bytes), never by a total read back.
+ *
+ *  - Documents.  Document d is d_utf8[o[d] .. o[d+1]) with o = d_offsets, int32 (offset_bytes = 4) or int64 (8), Arrow
+ *    style: [n_docs + 1] entries, o[0] may be > 0.  d_utf8 may have any alignment; the documents lie in [0, n_bytes).  The
+ *    kernels read the 16-byte blocks that hold [d_utf8, d_utf8 + n_bytes) and nothing else.
+ *  - Offsets are checked on the device.  A document with o[d] < 0, o[d] > o[d+1], o[d+1] > n_bytes or more than 1 GiB, or
+ *    that starts before an earlier offset of the array, gets status VPT_SENT_BAD_RANGE and 0 tokens; the others keep their
+ *    exact range.
+ *  - Outputs: d_token_offsets [n_docs + 1] (token r of document d is record d_token_offsets[d] + r; the last entry is the
+ *    total), d_n_tokens and d_status [n_docs], d_token_ends [max(n_bytes, 1)]: its first d_token_offsets[n_docs] entries
+ *    are written.  Tags (nullable, the predictor needs predict_tags): d_token_ids [n_bytes] and d_token_cands
+ *    [n_bytes * n_tags], as in vpt_token_spans (a model without tag slots: ids -1).  Tag scores are not returned.
+ *  - d_workspace: vpt_token_spans_dev_workspace_size(predictor, n_docs, n_bytes, tags) bytes of device scratch.
+ *  - Checked on the host, before anything is queued: NULL pointers, offset_bytes, the workspace size, the flags (as
+ *    vpt_token_spans), that every pointer is device memory of the predictor's device, and the batch limit: n_bytes and
+ *    n_docs at most 2^32 - 16 (32-bit character and token indexes of the tag kernels).
+ *  - n_docs == 0 writes d_token_offsets[0] = 0 and returns VPT_OK (the per-document outputs and the workspace may then be
+ *    NULL). */
+uint64_t vpt_token_spans_dev_workspace_size(const vpt_predictor* predictor, size_t n_docs, uint64_t n_bytes, int tags);
+int vpt_token_spans_dev(const vpt_predictor* predictor,
+                        const uint8_t* d_utf8, uint64_t n_bytes,
+                        const void* d_offsets, int offset_bytes,
+                        size_t n_docs, int no_norm, uint32_t wsconst_types,
+                        uint64_t* d_token_offsets,
+                        uint32_t* d_n_tokens, uint8_t* d_status,
+                        uint32_t* d_token_ends,
+                        int32_t* d_token_ids, uint8_t* d_token_cands,
+                        void* d_workspace, uint64_t workspace_bytes, void* cuda_stream);
 
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */

@@ -259,6 +259,32 @@ public:
         return r;
     }
 
+    /// Device buffers of `token_spans_dev` (see `vpt_token_spans_dev` for their sizes)
+    struct DeviceSpans {
+        uint64_t* token_offsets = nullptr;  // n_documents + 1
+        uint32_t* n_tokens = nullptr;
+        uint8_t* status = nullptr;
+        uint32_t* token_ends = nullptr;
+        int32_t* token_ids = nullptr;       // nullable: tags
+        uint8_t* token_cands = nullptr;
+        void* workspace = nullptr;          // token_spans_dev_workspace_size bytes
+        uint64_t workspace_bytes = 0;
+    };
+    /// bytes of device scratch `token_spans_dev` needs (vpt_token_spans_dev_workspace_size)
+    uint64_t token_spans_dev_workspace_size(size_t n_docs, uint64_t n_bytes, bool tags) const {
+        return vpt_token_spans_dev_workspace_size(h_, n_docs, n_bytes, tags ? 1 : 0);
+    }
+    /// `token_spans` for documents already in device memory (`vpt_token_spans_dev`): `d_offsets` holds n_docs + 1 int32
+    /// (offset_bytes 4) or int64 (8) offsets into `d_utf8`; all work is queued on `stream` (a cudaStream_t), nothing is
+    /// synchronised or allocated, so the call can be captured in a CUDA graph.
+    void token_spans_dev(const uint8_t* d_utf8, uint64_t n_bytes, const void* d_offsets, int offset_bytes, size_t n_docs,
+                         const DeviceSpans& out, bool no_norm = false, uint32_t wsconst_types = 0,
+                         void* stream = nullptr) const {
+        detail::check(vpt_token_spans_dev(h_, d_utf8, n_bytes, d_offsets, offset_bytes, n_docs, no_norm ? 1 : 0, wsconst_types,
+                                          out.token_offsets, out.n_tokens, out.status, out.token_ends, out.token_ids,
+                                          out.token_cands, out.workspace, out.workspace_bytes, stream));
+    }
+
     /// the longest tag score vector of the predictor's tokens (vpt_tag_score_len)
     size_t max_score_len() const {
         size_t m = 0;

@@ -14,7 +14,7 @@ import numpy as np
 
 __all__ = ["Model", "Predictor", "Sentence", "VaporettoError", "CharacterBoundary", "CharacterType", "lib", "build",
            "BatchResult", "build_blob", "shard_by_bytes", "LineStream", "SpansResult", "SpanToken", "Tokenizer",
-           "PatternMatchTagger"]
+           "PatternMatchTagger", "DeviceSpans"]
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("VPT_B200_LIBRARY") or os.path.join(_PKG, "libvaporetto_b200.so")  # (override: A/B builds)
@@ -141,6 +141,9 @@ ABI = [
                                                        C.POINTER(C.c_uint64), _P, C.c_size_t, C.POINTER(C.c_uint64)]),
     ("vpt_token_spans_tag_scores", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                              C.POINTER(C.c_uint64), _P, C.c_size_t, C.POINTER(C.c_uint64)]),
+    ("vpt_token_spans_dev_workspace_size", C.c_uint64, [_P, C.c_size_t, C.c_uint64, C.c_int]),
+    ("vpt_token_spans_dev", C.c_int, [_P, _P, C.c_uint64, _P, C.c_int, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P,
+                                      _P, _P, C.c_uint64, _P]),
 ]
 
 # vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
@@ -590,6 +593,47 @@ class Predictor:
             _attach_scores(r, self, sc[: nsc.value])
         return r
 
+    def token_spans_device(self, text, offsets, no_norm: bool = False, wsconst: str = "", tags: bool = False,
+                           stream=None) -> "DeviceSpans":
+        """token_spans for documents already in GPU memory (vpt_token_spans_dev): `text` is a 1-D torch.uint8 CUDA
+        tensor (any view of a larger buffer), `offsets` its n_docs + 1 int32 or int64 Arrow-style offsets on the same
+        device; document d is text[offsets[d]:offsets[d + 1]].  A cuDF / Arrow string column or a CuPy array comes in
+        without a copy through torch.as_tensor (the column's chars and offsets buffers).  The call is queued on `stream`
+        (default: torch.cuda.current_stream()), its workspace and outputs come from torch's caching allocator on that
+        stream, and it neither synchronises nor reads anything back: it is stream-ordered and can be captured in a CUDA
+        graph.  A document whose offsets are not a range inside the text has status 4 (VPT_SENT_BAD_RANGE) and no
+        tokens.  See DeviceSpans; DeviceSpans.to_host() gives what token_spans returns."""
+        import torch
+        if not isinstance(text, torch.Tensor) or text.dtype != torch.uint8 or text.dim() != 1 or not text.is_cuda:
+            raise VaporettoError(2, "InvalidArgumentError: text: must be a 1-D torch.uint8 CUDA tensor")
+        if (not isinstance(offsets, torch.Tensor) or offsets.dtype not in (torch.int32, torch.int64) or offsets.dim() != 1
+                or offsets.numel() < 1):
+            raise VaporettoError(2, "InvalidArgumentError: offsets: must be a 1-D int32 or int64 tensor of n_docs + 1")
+        if text.device != offsets.device or text.device.index != self.info["device"]:
+            raise VaporettoError(2, f"InvalidArgumentError: text/offsets: must be on the predictor's device "
+                                    f"cuda:{self.info['device']}")
+        mask = _wsconst_mask(wsconst)
+        dev = text.device
+        st = torch.cuda.current_stream(dev) if stream is None else stream
+        n, nb = offsets.numel() - 1, text.numel()
+        nt = self.n_tags if tags else 0
+        L = lib()
+        with torch.cuda.stream(st):
+            text, offsets = text.contiguous(), offsets.contiguous()
+            ws_bytes = L.vpt_token_spans_dev_workspace_size(self._h, n, nb, int(tags))
+            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+            tok_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            n_tokens = torch.empty(max(n, 1), dtype=torch.int32, device=dev)[:n]  # (an empty tensor has no pointer)
+            status = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)[:n]
+            ends = torch.empty(max(nb, 1), dtype=torch.int32, device=dev)  # a token has at least one byte
+            ids = torch.empty(max(nb, 1), dtype=torch.int32, device=dev) if tags else None
+            cands = torch.empty((max(nb, 1), nt), dtype=torch.uint8, device=dev) if tags else None
+            dp = lambda t: None if t is None else t.data_ptr()
+            _check(L.vpt_token_spans_dev(self._h, dp(text) if nb else None, nb, dp(offsets), offsets.element_size(), n,
+                                         int(no_norm), mask, dp(tok_off), dp(n_tokens), dp(status), dp(ends), dp(ids),
+                                         dp(cands) if nt else None, dp(ws), ws_bytes, st.cuda_stream))
+        return DeviceSpans(tok_off, n_tokens, status, ends, ids, cands, st, ws)
+
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
                     scores: bool = False, tag_scores: bool = False) -> "LineStream":
@@ -828,6 +872,30 @@ class SpansResult(_ScoredRecords):
         out[:1, 0] = 0
         out[1:, 0] = ends[:-1]
         return out
+
+
+class DeviceSpans:
+    """Result of Predictor.token_spans_device, torch tensors on the device, valid once the call's stream reaches them:
+    `token_offsets` (int64, n_docs + 1: the first token record of every document, the total last), `n_tokens` (int32) and
+    `status` (uint8, VPT_SENT_*; 4 = offsets out of range) per document, `token_ends` (int32, sized by the text's bytes:
+    its first token_offsets[-1] entries are the token ends), and with tags `token_ids` (int32) and `token_cands` (uint8
+    [bytes, n_tags]), sized like token_ends."""
+
+    def __init__(self, token_offsets, n_tokens, status, token_ends, token_ids, token_cands, stream, workspace):
+        self.token_offsets, self.n_tokens, self.status = token_offsets, n_tokens, status
+        self.token_ends, self.token_ids, self.token_cands = token_ends, token_ids, token_cands
+        self.stream = stream
+        self._workspace = workspace  # (kept with the outputs: the queued kernels use it)
+
+    def to_host(self) -> "SpansResult":
+        """Synchronises the stream and returns the SpansResult token_spans gives for the same documents."""
+        self.stream.synchronize()
+        k = int(self.token_offsets[-1].item())
+        host = lambda t, dt: t.cpu().numpy().view(dt)
+        return SpansResult(host(self.n_tokens, np.uint32), host(self.status, np.uint8),
+                           host(self.token_ends[:k], np.uint32),
+                           None if self.token_ids is None else host(self.token_ids[:k], np.int32),
+                           None if self.token_cands is None else host(self.token_cands[:k], np.uint8))
 
 
 class SpanToken:

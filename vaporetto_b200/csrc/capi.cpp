@@ -2555,6 +2555,81 @@ std::vector<std::pair<size_t, size_t>> span_chunks(const uint64_t* byte_offsets,
     return out;
 }
 
+// Device buffers of the span stage of vpt_token_spans and vpt_token_spans_dev
+struct SpanStage {
+    uint8_t* status8 = nullptr;
+    uint32_t* n_tokens = nullptr;
+    uint64_t* tok_base = nullptr;
+    uint32_t* tok_local = nullptr;
+    uint64_t* tok_blk = nullptr;
+    uint64_t* tok_total_host = nullptr;  // nullable (SpanArgs::tok_total_host)
+    uint32_t* token_ends = nullptr;
+    // tag prediction (tok_ids == nullptr: none), as TagArgs
+    int32_t* tok_ids = nullptr;
+    uint8_t* tok_cands = nullptr;
+    uint4* tok_desc = nullptr;
+    uint32_t* tok_work = nullptr;
+    uint64_t max_tokens = 0;
+    const TagScoreArgs* scores = nullptr;  // nullable
+};
+
+// The kernels of token_stream behind the scoring pass of the documents `a`: SplitLinebreaksFilter, the wsconst post-filters,
+// the token counts and their prefix, tags on the final boundaries (tokens looked up by their pre-filtered bytes, as
+// vpt_tokenize_lines_tags), token ends.  `tr` (nullable): the trace mark between the token counts and the tags.
+void launch_span_stage(const vpt_predictor* p, const BatchArgs& a, uint32_t wsconst_types, bool normalize, const SpanStage& b,
+                       cudaStream_t st, TraceEvents* tr) {
+    SpanArgs g;
+    g.text = a.text;
+    g.offsets = a.offsets;
+    g.n_sent = a.n_sent;
+    g.status = a.status;
+    g.n_chars = a.n_chars;
+    g.boundaries = a.boundaries;
+    g.bound_offsets = a.bound_offsets;
+    cuda_check(launch_split_linebreaks(g, st), "launch(split linebreaks)");
+    TokArgs t;
+    t.text = a.text;
+    t.offsets = a.offsets;
+    t.n_sent = a.n_sent;
+    t.status = a.status;
+    t.n_chars = a.n_chars;
+    t.boundaries = a.boundaries;
+    t.bound_offsets = a.bound_offsets;
+    cuda_check(launch_wsconst(t, a.boundaries, wsconst_types, normalize, st), "launch(wsconst)");
+    if (wsconst_types & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
+    g.status8 = b.status8;
+    g.n_tokens = b.n_tokens;
+    g.tok_base = b.tok_base;
+    g.tok_local = b.tok_local;
+    g.tok_blk = b.tok_blk;
+    g.tok_total_host = b.tok_total_host;
+    cuda_check(launch_span_count(g, st), "launch(span count)");
+    if (tr) tr->mark_sub(1, st);  // after the filters and the token counts
+    if (b.tok_ids) {
+        TagArgs ta;
+        ta.text = a.text;
+        ta.offsets = a.offsets;
+        ta.n_sent = a.n_sent;
+        ta.status = a.status;
+        ta.boundaries = a.boundaries;
+        ta.bound_offsets = a.bound_offsets;
+        ta.char_offsets = a.char_offsets;
+        ta.char_states = p->dt.char_rels ? a.char_states : nullptr;
+        ta.type_states = p->dt.type_rels ? a.type_states : nullptr;
+        ta.tok_base = g.tok_base;
+        ta.tok_ids = b.tok_ids;
+        ta.tok_cands = b.tok_cands;
+        ta.tok_desc = b.tok_desc;
+        ta.max_tokens = b.max_tokens;
+        ta.tok_work = b.tok_work;
+        ta.text_base = 0;
+        ta.norm = normalize ? 1 : 0;
+        cuda_check(launch_tags(p->dt, ta, st, b.scores), "launch(tags)");
+    }
+    g.token_ends = b.token_ends;
+    cuda_check(launch_token_ends(g, st), "launch(token ends)");
+}
+
 }  // namespace
 
 int vpt_token_spans(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_docs, int no_norm,
@@ -2648,77 +2723,42 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
             a.char_states = static_cast<uint32_t*>(s.d_cst);
             a.type_states = static_cast<uint32_t*>(s.d_tst);
         }
-        // (chunk-local offsets: bound_base / char_base stay 0)
-        if (pipeline_trace()) ch.tr.mark(1, st);
-        cuda_check(launch_score(dm, a, st), "launch(score)");
-        if (pipeline_trace()) ch.tr.mark_sub(0, st);  // after the scoring kernel
-        SpanArgs g;
-        g.text = a.text;
-        g.offsets = a.offsets;
-        g.n_sent = ch.n;
-        g.status = a.status;
-        g.n_chars = a.n_chars;
-        g.boundaries = a.boundaries;
-        g.bound_offsets = a.bound_offsets;
-        cuda_check(launch_split_linebreaks(g, st), "launch(split linebreaks)");
-        TokArgs t;
-        t.text = a.text;
-        t.offsets = a.offsets;
-        t.n_sent = ch.n;
-        t.status = a.status;
-        t.n_chars = a.n_chars;
-        t.boundaries = a.boundaries;
-        t.bound_offsets = a.bound_offsets;
-        cuda_check(launch_wsconst(t, a.boundaries, wsconst_types, normalize, st), "launch(wsconst)");
-        if (wsconst_types & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
         Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
         Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * ch.n + 16);
         Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (ch.n + 1) + 16);
         Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * ch.n + 16);
         Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (ch.n / kSpanDocs + 4));
-        g.status8 = static_cast<uint8_t*>(s.d_st8);
-        g.n_tokens = static_cast<uint32_t*>(s.d_ntok);
-        g.tok_base = static_cast<uint64_t*>(s.d_tokbase);
-        g.tok_local = static_cast<uint32_t*>(s.d_toklocal);
-        g.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
-        g.tok_total_host = &s.h_totals[4];
+        Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
+        SpanStage b;
+        b.status8 = static_cast<uint8_t*>(s.d_st8);
+        b.n_tokens = static_cast<uint32_t*>(s.d_ntok);
+        b.tok_base = static_cast<uint64_t*>(s.d_tokbase);
+        b.tok_local = static_cast<uint32_t*>(s.d_toklocal);
+        b.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+        b.tok_total_host = &s.h_totals[4];
         s.h_totals[4] = 0;
-        cuda_check(launch_span_count(g, st), "launch(span count)");
-        if (pipeline_trace()) ch.tr.mark_sub(1, st);  // after the filters and the token counts
+        b.token_ends = static_cast<uint32_t*>(s.d_ends);
+        TagScoreArgs sc;
         if (tags) {
-            // tag prediction on the final boundaries, tokens looked up by their pre-filtered bytes (as vpt_tokenize_lines_tags)
             Scratch::ensure(s.d_tok, s.tok_cap, 4 * nc + 16);
             Scratch::ensure(s.d_cand, s.cand_cap, nc * std::max<size_t>(nt, 1) + 16);
             Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * nc + 16);
             Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nc + 32);
-            TagArgs ta;
-            ta.text = a.text;
-            ta.offsets = a.offsets;
-            ta.n_sent = ch.n;
-            ta.status = a.status;
-            ta.boundaries = a.boundaries;
-            ta.bound_offsets = a.bound_offsets;
-            ta.char_offsets = a.char_offsets;
-            ta.char_states = p->dt.char_rels ? a.char_states : nullptr;
-            ta.type_states = p->dt.type_rels ? a.type_states : nullptr;
-            ta.tok_base = g.tok_base;
-            ta.tok_ids = static_cast<int32_t*>(s.d_tok);
-            ta.tok_cands = static_cast<uint8_t*>(s.d_cand);
-            ta.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-            ta.max_tokens = nc;
-            ta.tok_work = static_cast<uint32_t*>(s.d_tokwork);
-            ta.text_base = 0;
-            ta.norm = normalize ? 1 : 0;
+            b.tok_ids = static_cast<int32_t*>(s.d_tok);
+            b.tok_cands = static_cast<uint8_t*>(s.d_cand);
+            b.tok_desc = static_cast<uint4*>(s.d_tokdesc);
+            b.tok_work = static_cast<uint32_t*>(s.d_tokwork);
+            b.max_tokens = nc;
             if (want_scores) {
-                const TagScoreArgs sc = bind_tag_scores(s, nc, score_len);
-                cuda_check(launch_tags(p->dt, ta, st, &sc), "launch(tags)");
-            } else {
-                cuda_check(launch_tags(p->dt, ta, st), "launch(tags)");
+                sc = bind_tag_scores(s, nc, score_len);
+                b.scores = &sc;
             }
         }
-        Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
-        g.token_ends = static_cast<uint32_t*>(s.d_ends);
-        cuda_check(launch_token_ends(g, st), "launch(token ends)");
+        // (chunk-local offsets: bound_base / char_base stay 0)
+        if (pipeline_trace()) ch.tr.mark(1, st);
+        cuda_check(launch_score(dm, a, st), "launch(score)");
+        if (pipeline_trace()) ch.tr.mark_sub(0, st);  // after the scoring kernel
+        launch_span_stage(p, a, wsconst_types, normalize, b, st, pipeline_trace() ? &ch.tr : nullptr);
         if (pipeline_trace()) ch.tr.mark(2, st);
         cuda_check(cudaEventRecord(cc.kernels, st), "cudaEventRecord");
         cc.issued = true;
@@ -2775,6 +2815,150 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
         throw Error(kInvalidArgument, "InvalidArgumentError: token_capacity: too small for the batch");
     }
     if (want_tags && !tags) std::fill(token_ids_out, token_ids_out + tok_total, -1);  // a model without tag slots
+    return kOk;
+    VPT_API_END
+}
+
+namespace {
+
+// Batch limit of vpt_token_spans_dev, for n_bytes and n_docs: the tag kernels index characters and token records of the
+// whole batch with 32 bits (TagArgs::tok_desc .z, TagArgs::tok_work), and tokens <= characters <= bytes (+ 15 of shift)
+constexpr uint64_t kMaxSpansDevBatch = (uint64_t(1) << 32) - 16;
+
+// Scratch of vpt_token_spans_dev in the caller's workspace: byte offsets of every buffer; 0 size = not used
+struct SpansDevLayout {
+    size_t off, bad, dblk, ws, status, boff, coff, bounds, scores, cst, tst, tokdesc, tokwork, toklocal, tokblk, total;
+};
+SpansDevLayout spans_dev_layout(const vpt_predictor* p, uint64_t n_docs, uint64_t n_bytes, bool tags) {
+    SpansDevLayout l;
+    const uint64_t n = n_docs, b = n_bytes;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o = align_up(o + bytes, 256); return at; };
+    l.off = take(8 * (n + 1));
+    l.bad = take(n);
+    l.dblk = take(8 * doc_offsets_blocks(n));
+    l.ws = take(workspace_layout(n).total);
+    l.status = take(4 * n);
+    l.boff = take(8 * (n + 1));
+    l.coff = tags ? take(8 * (n + 1)) : 0;
+    l.bounds = take(b + 4);  // (the span kernels read boundaries as words)
+    l.scores = scores_optional(p->dm) ? 0 : take(4 * b + 4);
+    l.cst = tags ? take(4 * b + 4) : 0;
+    l.tst = tags ? take(4 * b + 4) : 0;
+    l.tokdesc = tags ? take(16 * b + 16) : 0;
+    l.tokwork = tags ? take(4 * b + 32) : 0;
+    l.toklocal = take(4 * n);
+    l.tokblk = take(8 * (n / kSpanDocs + 4));
+    l.total = o + 256;
+    return l;
+}
+
+// `ptr` is device memory of the predictor's device (cudaPointerGetAttributes: no stream work, allowed under capture)
+void require_device_ptr(const vpt_predictor* p, const void* ptr, const char* name) {
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, ptr) != cudaSuccess) {
+        cudaGetLastError();
+        throw Error(kInvalidArgument, std::string("InvalidArgumentError: ") + name + ": not device memory");
+    }
+    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != p->device)
+        throw Error(kInvalidArgument, std::string("InvalidArgumentError: ") + name +
+                                          ": must be device memory of the predictor's device " + std::to_string(p->device));
+}
+
+}  // namespace
+
+uint64_t vpt_token_spans_dev_workspace_size(const vpt_predictor* p, size_t n_docs, uint64_t n_bytes, int tags) {
+    if (!p || p->device < 0) return 0;
+    return spans_dev_layout(p, n_docs, n_bytes, tags != 0 && p->n_tags > 0).total;
+}
+
+int vpt_token_spans_dev(const vpt_predictor* p, const uint8_t* d_utf8, uint64_t n_bytes, const void* d_offsets,
+                        int offset_bytes, size_t n_docs, int no_norm, uint32_t wsconst_types, uint64_t* d_token_offsets,
+                        uint32_t* d_n_tokens, uint8_t* d_status, uint32_t* d_token_ends, int32_t* d_token_ids,
+                        uint8_t* d_token_cands, void* d_workspace, uint64_t workspace_bytes, void* cuda_stream) {
+    VPT_API_BEGIN
+    // Every check reads the arguments only: nothing here synchronises, allocates or touches the device's data
+    const bool want_tags = d_token_ids != nullptr || d_token_cands != nullptr;
+    const bool tags = check_lines_flags(p, wsconst_types, want_tags);  // false with n_tags == 0: every token id is -1
+    if (want_tags && (!d_token_ids || (tags && !d_token_cands)))
+        throw Error(kInvalidArgument, "InvalidArgumentError: d_token_ids/d_token_cands: must not be NULL");
+    if (offset_bytes != 4 && offset_bytes != 8)
+        throw Error(kInvalidArgument, "InvalidArgumentError: offset_bytes: must be 4 (int32) or 8 (int64)");
+    if (!d_offsets || !d_token_offsets || (n_docs > 0 && (!d_n_tokens || !d_status || !d_token_ends)))
+        throw Error(kInvalidArgument, "InvalidArgumentError: device buffers: must not be NULL");
+    if (n_bytes > 0 && !d_utf8) throw Error(kInvalidArgument, "InvalidArgumentError: d_utf8: must not be NULL");
+    if (n_bytes > kMaxSpansDevBatch || n_docs > kMaxSpansDevBatch)
+        throw Error(kInvalidArgument, "InvalidArgumentError: n_bytes/n_docs: over the batch limit of 2^32 - 16 (32-bit "
+                                      "character and token indexes of the tag kernels)");
+    const SpansDevLayout l = spans_dev_layout(p, n_docs, n_bytes, tags);
+    if (n_docs > 0 && (!d_workspace || workspace_bytes < l.total))
+        throw Error(kInvalidArgument, "InvalidArgumentError: workspace: too small (vpt_token_spans_dev_workspace_size)");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    if (n_bytes > 0) require_device_ptr(p, d_utf8, "d_utf8");
+    require_device_ptr(p, d_offsets, "d_offsets");
+    require_device_ptr(p, d_token_offsets, "d_token_offsets");
+    if (n_docs > 0) {
+        require_device_ptr(p, d_n_tokens, "d_n_tokens");
+        require_device_ptr(p, d_status, "d_status");
+        require_device_ptr(p, d_token_ends, "d_token_ends");
+        require_device_ptr(p, d_workspace, "d_workspace");
+    }
+    if (d_token_ids) require_device_ptr(p, d_token_ids, "d_token_ids");
+    if (tags) require_device_ptr(p, d_token_cands, "d_token_cands");
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    if (want_tags && !tags && n_bytes)  // a model without tag slots
+        cuda_check(cudaMemsetAsync(d_token_ids, 0xFF, 4 * n_bytes, st), "memset(token ids)");
+    if (n_docs == 0) {
+        cuda_check(cudaMemsetAsync(d_token_offsets, 0, 8, st), "memset(token offsets)");
+        return kOk;
+    }
+    uint8_t* w = static_cast<uint8_t*>(d_workspace);
+    const bool normalize = no_norm == 0;
+    DevModel dm = p->dm;
+    dm.kytea_norm = normalize ? 1 : 0;
+
+    // the caller's offsets -> offsets into the text rounded down to 16 bytes, and the documents out of range
+    const uintptr_t text_addr = reinterpret_cast<uintptr_t>(d_utf8);
+    DocArgs da;
+    da.offsets = d_offsets;
+    da.wide = offset_bytes == 8;
+    da.n_docs = n_docs;
+    da.n_bytes = n_bytes;
+    da.shift = uint32_t(text_addr & 15);
+    da.out = reinterpret_cast<uint64_t*>(w + l.off);
+    da.bad = w + l.bad;
+    da.blk = reinterpret_cast<uint64_t*>(w + l.dblk);
+    cuda_check(launch_doc_offsets(da, st), "launch(doc offsets)");
+
+    BatchArgs a;
+    a.text = reinterpret_cast<const uint8_t*>(text_addr & ~uintptr_t(15));
+    a.offsets = da.out;
+    a.n_sent = n_docs;
+    bind_workspace(a, w + l.ws, n_docs);
+    a.status = reinterpret_cast<int32_t*>(w + l.status);
+    a.bound_offsets = reinterpret_cast<uint64_t*>(w + l.boff);
+    a.boundaries = w + l.bounds;
+    a.scores = l.scores ? reinterpret_cast<int32_t*>(w + l.scores) : nullptr;
+    SpanStage b;
+    b.status8 = d_status;
+    b.n_tokens = d_n_tokens;
+    b.tok_base = d_token_offsets;
+    b.tok_local = reinterpret_cast<uint32_t*>(w + l.toklocal);
+    b.tok_blk = reinterpret_cast<uint64_t*>(w + l.tokblk);
+    b.token_ends = d_token_ends;
+    if (tags) {
+        a.char_offsets = reinterpret_cast<uint64_t*>(w + l.coff);
+        a.char_states = reinterpret_cast<uint32_t*>(w + l.cst);
+        a.type_states = reinterpret_cast<uint32_t*>(w + l.tst);
+        b.tok_ids = d_token_ids;
+        b.tok_cands = d_token_cands;
+        b.tok_desc = reinterpret_cast<uint4*>(w + l.tokdesc);
+        b.tok_work = reinterpret_cast<uint32_t*>(w + l.tokwork);
+        b.max_tokens = n_bytes;
+    }
+    cuda_check(launch_batch(dm, a, st), "launch(batch)");
+    cuda_check(launch_doc_status(da, a.status, st), "launch(doc status)");
+    launch_span_stage(p, a, wsconst_types, normalize, b, st, nullptr);
     return kOk;
     VPT_API_END
 }

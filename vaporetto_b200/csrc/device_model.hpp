@@ -230,4 +230,21 @@ cudaError_t launch_span_count(const SpanArgs& a, cudaStream_t stream);
 // the byte offset of every token's exclusive end, relative to its document
 cudaError_t launch_token_ends(const SpanArgs& a, cudaStream_t stream);
 
+// ---- doc_offsets.cu: the caller's device offsets of vpt_token_spans_dev (doc_offsets.hpp) ----------------------------
+struct DocArgs {
+    const void* offsets = nullptr;  // [n_docs + 1] int64 (wide) or int32, as the caller passed them
+    int32_t wide = 0;
+    uint64_t n_docs = 0;
+    uint64_t n_bytes = 0;
+    uint32_t shift = 0;             // the text's address mod 16
+    uint64_t* out = nullptr;        // [n_docs + 1] rebased offsets into the text rounded down to 16 bytes
+    uint8_t* bad = nullptr;         // [n_docs] 1: the document is out of range (VPT_SENT_BAD_RANGE)
+    uint64_t* blk = nullptr;        // [doc_offsets_blocks(n_docs)] scratch
+};
+uint64_t doc_offsets_blocks(uint64_t n_docs);
+// out and bad from the caller's offsets
+cudaError_t launch_doc_offsets(const DocArgs& a, cudaStream_t stream);
+// status[d] = VPT_SENT_BAD_RANGE for every flagged document (after the scoring pass, before launch_split_linebreaks)
+cudaError_t launch_doc_status(const DocArgs& a, int32_t* status, cudaStream_t stream);
+
 }  // namespace vpt
