@@ -389,6 +389,51 @@ void bind_workspace(BatchArgs& a, void* ws, size_t n) {
     a.ticket = reinterpret_cast<uint32_t*>(b + l.ticket);
 }
 
+// The fields of TagArgs that come from the scoring pass `a` (the pattern-id states only where the model's tags read them)
+TagArgs tag_args(const DevTags& dt, const BatchArgs& a) {
+    TagArgs t;
+    t.text = a.text;
+    t.offsets = a.offsets;
+    t.trims = a.trims;
+    t.n_sent = a.n_sent;
+    t.status = a.status;
+    t.boundaries = a.boundaries;
+    t.bound_offsets = a.bound_offsets;
+    t.char_offsets = a.char_offsets;
+    t.char_states = dt.char_rels ? a.char_states : nullptr;
+    t.type_states = dt.type_rels ? a.type_states : nullptr;
+    return t;
+}
+
+// Ensures the per-token tag records of at most `m` tokens and binds them (tok_ids, tok_cands, tok_desc, tok_work,
+// max_tokens) into `r`, a TagArgs or a SpanStage
+template <class R>
+void bind_token_records(const vpt_predictor& p, Scratch& s, R& r, uint64_t m) {
+    Scratch::ensure(s.d_tok, s.tok_cap, 4 * m + 16);
+    Scratch::ensure(s.d_cand, s.cand_cap, m * std::max<size_t>(p.n_tags, 1) + 16);
+    Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * m + 16);
+    Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * m + 32);
+    r.tok_ids = static_cast<int32_t*>(s.d_tok);
+    r.tok_cands = static_cast<uint8_t*>(s.d_cand);
+    r.tok_desc = static_cast<uint4*>(s.d_tokdesc);
+    r.tok_work = static_cast<uint32_t*>(s.d_tokwork);
+    r.max_tokens = m;
+}
+
+// Ensures the token counts of `n` sentences, their prefix and its scratch and binds them (n_tokens, tok_base, tok_local,
+// tok_blk) into `k`, a CompactArgs or a SpanStage; the prefix of both kernels runs in blocks of kSpanDocs sentences
+template <class K>
+void bind_token_counts(Scratch& s, K& k, size_t n) {
+    Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * n + 16);
+    Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (n + 1) + 16);
+    Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * n + 16);
+    Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (n / kSpanDocs + 4));
+    k.n_tokens = static_cast<uint32_t*>(s.d_ntok);
+    k.tok_base = static_cast<uint64_t*>(s.d_tokbase);
+    k.tok_local = static_cast<uint32_t*>(s.d_toklocal);
+    k.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+}
+
 // ---- host-side text helpers ------------------------------------------------------------------------
 
 // Sentence::parse_raw checks (reference sentence.rs:160-196)
@@ -800,6 +845,21 @@ std::vector<size_t> ramp_schedule(size_t total, size_t big, size_t small_up, siz
     return out;
 }
 
+// Pipeline chunks of vpt_predict_batch and vpt_predict_batch_compact as (first sentence, sentences): the ramp schedule
+// over chunk_sentences()
+std::vector<std::pair<size_t, size_t>> sentence_chunks(const uint64_t* byte_offsets, size_t n_sent) {
+    const size_t cs = chunk_sentences();
+    std::vector<std::pair<size_t, size_t>> out;
+    size_t lo = 0;
+    for (size_t sz : ramp_schedule(n_sent, cs, cs / 8, cs / 4)) {
+        if (byte_offsets[lo + sz] < byte_offsets[lo])
+            throw Error(kInvalidArgument, "InvalidArgumentError: byte_offsets: must be non-decreasing");
+        out.emplace_back(lo, sz);
+        lo += sz;
+    }
+    return out;
+}
+
 // Pipeline trace (env VPT_TRACE=1): per chunk, CUDA-event times of copy-in end, kernels start / end and copy-out
 // end are printed to stderr when the call returns.
 bool pipeline_trace() {
@@ -837,10 +897,14 @@ struct TraceEvents {
     }
 };
 
+constexpr size_t kRingDepth = 4;  // chunks in flight in the batch ring and the line ring
+
 struct ChunkState {
     size_t s_lo = 0, n = 0;       // sentence range
     uint64_t byte_lo = 0, nbytes = 0;
-    cudaEvent_t counted = nullptr;
+    uint64_t nb = 0, nc = 0;      // boundaries and characters, from the count pass
+    cudaEvent_t counted = nullptr, kernels = nullptr;
+    bool issued = false;          // the chunk's kernels are queued
     TraceEvents tr;
     BatchArgs a;
 };
@@ -881,6 +945,92 @@ void chunk_count(Scratch& s, ChunkState& ch, const uint8_t* utf8, const uint64_t
     cuda_check(cudaEventRecord(ch.counted, st), "cudaEventRecord");
 }
 
+// ---- the batch ring: the chunk pipeline of vpt_predict_batch, vpt_predict_batch_compact* and vpt_token_spans* --------
+//
+// Every chunk of sentences (or documents) goes through chunk_count (copy-in, count pass), then its caller's `issue`
+// (output bindings and kernels on the scratch's stream), then its caller's `copy_out` (D2H copies on stream_out).  Chunk c
+// runs on lease c % kRingDepth, so the copy-in, kernels and copy-out of neighbouring chunks overlap; a chunk's kernels
+// wait for the copy-out of its lease's previous chunk (ev_out, see chunk_count).  A call whose copy-out needs totals
+// its kernels wrote (`wait_for_kernels`) copies each chunk out one step later, after a host wait for its kernels, and
+// counts kRingDepth - 2 chunks ahead; otherwise a chunk is copied out in the step that issues it, and the count pass runs
+// kRingDepth - 1 chunks ahead.
+struct BatchRing {
+    // returns false when it skipped the chunk (an output overflowed): no kernels, no copy-out
+    using Issue = std::function<bool(size_t c, ChunkState& ch, Scratch& s)>;
+    using CopyOut = std::function<void(size_t c, ChunkState& ch, Scratch& s, cudaStream_t stream_out)>;
+    const char* const label;      // of the trace lines
+    const char* const sync_what;  // of the final check of the kernels' streams
+    std::vector<ChunkState> chunks;
+    std::unique_ptr<ScratchLease> lease[kRingDepth];
+
+    // `cuts`: (first sentence, sentences) of every chunk, in order
+    BatchRing(const vpt_predictor& p, const char* what, const char* sync, const uint64_t* byte_offsets,
+              const std::vector<std::pair<size_t, size_t>>& cuts)
+        : label(what), sync_what(sync), chunks(cuts.size()) {
+        for (size_t c = 0; c < cuts.size(); ++c) {
+            ChunkState& ch = chunks[c];
+            ch.s_lo = cuts[c].first;
+            ch.n = cuts[c].second;
+            ch.byte_lo = byte_offsets[ch.s_lo];
+            ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
+        }
+        for (size_t i = 0; i < kRingDepth && i < chunks.size(); ++i) lease[i].reset(new ScratchLease(p));
+    }
+
+    ~BatchRing() {
+        for (ChunkState& ch : chunks) {
+            if (ch.counted) cudaEventDestroy(ch.counted);
+            if (ch.kernels) cudaEventDestroy(ch.kernels);
+            ch.tr.destroy();
+        }
+    }
+
+    Scratch& scratch(size_t c) { return *lease[c % kRingDepth]->s; }
+
+    // The whole batch through the ring.  The final synchronisation is checked: a failed copy-out is an error of the
+    // call, not left to the leases' release.
+    void run(const uint8_t* utf8, const uint64_t* byte_offsets, bool wait_for_kernels, const Issue& issue,
+             const CopyOut& copy_out) {
+        const size_t nchunks = chunks.size();
+        const size_t ahead = wait_for_kernels ? kRingDepth - 2 : kRingDepth - 1;
+        const size_t behind = wait_for_kernels ? 1 : 0;
+        const bool trace = pipeline_trace();
+        for (size_t c = 0; c < std::min(ahead, nchunks); ++c) chunk_count(scratch(c), chunks[c], utf8, byte_offsets);
+        for (size_t step = 0; step < nchunks + 1; ++step) {
+            if (step + ahead < nchunks) chunk_count(scratch(step + ahead), chunks[step + ahead], utf8, byte_offsets);
+            if (step < nchunks) {
+                ChunkState& ch = chunks[step];
+                Scratch& s = scratch(step);
+                cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
+                ch.nb = s.h_totals[0];
+                ch.nc = s.h_totals[1];
+                ch.issued = issue(step, ch, s);
+                if (ch.issued) {
+                    if (trace) ch.tr.mark(2, s.stream);
+                    if (!ch.kernels) cuda_check(cudaEventCreateWithFlags(&ch.kernels, cudaEventDisableTiming), "cudaEventCreate");
+                    cuda_check(cudaEventRecord(ch.kernels, s.stream), "cudaEventRecord");
+                }
+            }
+            if (step < behind || step - behind >= nchunks || !chunks[step - behind].issued) continue;
+            const size_t c = step - behind;
+            ChunkState& ch = chunks[c];
+            Scratch& s = scratch(c);
+            if (wait_for_kernels) cuda_check(cudaEventSynchronize(ch.kernels), "sync(kernels)");
+            cuda_check(cudaStreamWaitEvent(s.stream_out, ch.kernels, 0), "cudaStreamWaitEvent");
+            copy_out(c, ch, s, s.stream_out);
+            cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
+            if (trace) ch.tr.mark(3, s.stream_out);
+        }
+        for (const std::unique_ptr<ScratchLease>& l : lease)
+            if (l) {
+                cuda_check(cudaStreamSynchronize(l->s->stream), sync_what);
+                cuda_check(cudaStreamSynchronize(l->s->stream_out), "sync(copy-out)");
+            }
+        if (trace)
+            for (size_t c = 0; c < nchunks; ++c) chunks[c].tr.print(label, c, chunks[c].n, chunks[0].tr);
+    }
+};
+
 }  // namespace
 
 int vpt_predict_batch(const vpt_predictor* p, const uint8_t* utf8, const uint64_t* byte_offsets, size_t n_sent,
@@ -901,87 +1051,54 @@ int vpt_predict_batch(const vpt_predictor* p, const uint8_t* utf8, const uint64_
         throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
 
-    // The batch is cut into chunks that flow through three streams so that the H2D copy of chunk c+2, the
-    // kernels of chunk c+1 and the D2H copy of chunk c overlap.  Each chunk is an independent batch on the
-    // device; its output offsets are rebased with the running totals (known on the host after its count pass).
-    const size_t kChunkSentences = chunk_sentences();
-    const std::vector<size_t> sizes = ramp_schedule(n_sent, kChunkSentences, kChunkSentences / 8, kChunkSentences / 4);
-    const size_t nchunks = sizes.size();
-    constexpr int kDepth = 4;
-    std::unique_ptr<ScratchLease> lease[kDepth];
-    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
-    std::vector<ChunkState> chunks(nchunks);
-    struct EventGuard {
-        std::vector<ChunkState>& c;
-        ~EventGuard() { for (auto& x : c) { if (x.counted) cudaEventDestroy(x.counted); x.tr.destroy(); } }
-    } guard{chunks};
-    for (size_t c = 0, lo = 0; c < nchunks; lo += sizes[c], ++c) {
-        ChunkState& ch = chunks[c];
-        ch.s_lo = lo;
-        ch.n = sizes[c];
-        ch.byte_lo = byte_offsets[ch.s_lo];
-        if (byte_offsets[ch.s_lo + ch.n] < ch.byte_lo)
-            throw Error(kInvalidArgument, "InvalidArgumentError: byte_offsets: must be non-decreasing");
-        ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
-    }
+    // The batch is cut into chunks that flow through the batch ring, so that the H2D copy of chunk c+2, the kernels of
+    // chunk c+1 and the D2H copy of chunk c overlap.  Each chunk is an independent batch on the device; its output
+    // offsets are rebased with the running totals (known on the host after its count pass).
+    BatchRing ring(*p, "batch", "sync(score)", byte_offsets, sentence_chunks(byte_offsets, n_sent));
+    const size_t nchunks = ring.chunks.size();
     const bool want_states = char_states_out || type_states_out;
     uint64_t nb_total = 0, nc_total = 0;
     bool overflow = false;
-    constexpr size_t kAhead = kDepth - 1;  // chunks whose copy-in + count pass are issued ahead of the scoring
-    for (size_t c = 0; c < std::min<size_t>(kAhead, nchunks); ++c) chunk_count(*lease[c % kDepth]->s, chunks[c], utf8, byte_offsets);
-    for (size_t c = 0; c < nchunks; ++c) {
-        ChunkState& ch = chunks[c];
-        Scratch& s = *lease[c % kDepth]->s;
+    auto issue = [&](size_t, ChunkState& ch, Scratch& s) {
         cudaStream_t st = s.stream;
-        cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
-        const uint64_t nb = s.h_totals[0], nc = s.h_totals[1];
+        const uint64_t nb = ch.nb, nc = ch.nc;
         if (nb_total + nb > out_capacity || (nb && !boundaries_out) || (want_states && nc_total + nc > states_capacity))
             overflow = true;
-        if (!overflow) {
-            BatchArgs& a = ch.a;
-            Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
-            a.scores = nullptr;  // boundaries only, when the caller wants no scores and the kernel can skip them
-            if (scores_out || !scores_optional(p->dm)) {
-                Scratch::ensure(s.d_scores, s.scores_cap, 4 * nb + 4);
-                a.scores = static_cast<int32_t*>(s.d_scores);
-            }
-            a.boundaries = static_cast<uint8_t*>(s.d_bounds);
-            if (char_states_out) { Scratch::ensure(s.d_cst, s.cst_cap, 4 * nc + 4); a.char_states = static_cast<uint32_t*>(s.d_cst); }
-            if (type_states_out) { Scratch::ensure(s.d_tst, s.tst_cap, 4 * nc + 4); a.type_states = static_cast<uint32_t*>(s.d_tst); }
-            a.bound_base = nb_total;
-            a.char_base = nc_total;
-            if (pipeline_trace()) ch.tr.mark(1, st);
-            cuda_check(launch_score(p->dm, a, st), "launch(score)");
-            if (pipeline_trace()) ch.tr.mark(2, st);
-            cuda_check(cudaEventRecord(s.ev_kernels, st), "cudaEventRecord");
-            cudaStream_t so = s.stream_out;
-            cuda_check(cudaStreamWaitEvent(so, s.ev_kernels, 0), "cudaStreamWaitEvent");
-            if (nb) {
-                if (scores_out) cuda_check(cudaMemcpyAsync(scores_out + nb_total, s.d_scores, 4 * nb, cudaMemcpyDeviceToHost, so), "D2H(scores)");
-                cuda_check(cudaMemcpyAsync(boundaries_out + nb_total, s.d_bounds, nb, cudaMemcpyDeviceToHost, so), "D2H(boundaries)");
-            }
-            // the last element of a chunk's offsets is the first of the next chunk's: copy n (+1 for the last chunk)
-            const size_t noff = ch.n + (c + 1 == nchunks ? 1 : 0);
-            cuda_check(cudaMemcpyAsync(bound_offsets_out + ch.s_lo, s.d_boff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
-            if (char_offsets_out)
-                cuda_check(cudaMemcpyAsync(char_offsets_out + ch.s_lo, s.d_coff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
-            if (status_out) cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_status, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
-            if (nc && char_states_out) cuda_check(cudaMemcpyAsync(char_states_out + nc_total, s.d_cst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
-            if (nc && type_states_out) cuda_check(cudaMemcpyAsync(type_states_out + nc_total, s.d_tst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
-            cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
-            if (pipeline_trace()) ch.tr.mark(3, so);
-        }
+        BatchArgs& a = ch.a;
+        a.bound_base = nb_total;
+        a.char_base = nc_total;
         nb_total += nb;
         nc_total += nc;
-        if (c + kAhead < nchunks) chunk_count(*lease[(c + kAhead) % kDepth]->s, chunks[c + kAhead], utf8, byte_offsets);
-    }
-    for (int i = 0; i < kDepth; ++i)
-        if (lease[i]) {
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(score)");
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
+        if (overflow) return false;
+        Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
+        a.scores = nullptr;  // boundaries only, when the caller wants no scores and the kernel can skip them
+        if (scores_out || !scores_optional(p->dm)) {
+            Scratch::ensure(s.d_scores, s.scores_cap, 4 * nb + 4);
+            a.scores = static_cast<int32_t*>(s.d_scores);
         }
-    if (pipeline_trace())
-        for (size_t c = 0; c < nchunks; ++c) chunks[c].tr.print("batch", c, chunks[c].n, chunks[0].tr);
+        a.boundaries = static_cast<uint8_t*>(s.d_bounds);
+        if (char_states_out) { Scratch::ensure(s.d_cst, s.cst_cap, 4 * nc + 4); a.char_states = static_cast<uint32_t*>(s.d_cst); }
+        if (type_states_out) { Scratch::ensure(s.d_tst, s.tst_cap, 4 * nc + 4); a.type_states = static_cast<uint32_t*>(s.d_tst); }
+        if (pipeline_trace()) ch.tr.mark(1, st);
+        cuda_check(launch_score(p->dm, a, st), "launch(score)");
+        return true;
+    };
+    auto copy_out = [&](size_t c, ChunkState& ch, Scratch& s, cudaStream_t so) {
+        const uint64_t nb = ch.nb, nc = ch.nc, b0 = ch.a.bound_base, c0 = ch.a.char_base;
+        if (nb) {
+            if (scores_out) cuda_check(cudaMemcpyAsync(scores_out + b0, s.d_scores, 4 * nb, cudaMemcpyDeviceToHost, so), "D2H(scores)");
+            cuda_check(cudaMemcpyAsync(boundaries_out + b0, s.d_bounds, nb, cudaMemcpyDeviceToHost, so), "D2H(boundaries)");
+        }
+        // the last element of a chunk's offsets is the first of the next chunk's: copy n (+1 for the last chunk)
+        const size_t noff = ch.n + (c + 1 == nchunks ? 1 : 0);
+        cuda_check(cudaMemcpyAsync(bound_offsets_out + ch.s_lo, s.d_boff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
+        if (char_offsets_out)
+            cuda_check(cudaMemcpyAsync(char_offsets_out + ch.s_lo, s.d_coff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
+        if (status_out) cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_status, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
+        if (nc && char_states_out) cuda_check(cudaMemcpyAsync(char_states_out + c0, s.d_cst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
+        if (nc && type_states_out) cuda_check(cudaMemcpyAsync(type_states_out + c0, s.d_tst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
+    };
+    ring.run(utf8, byte_offsets, false, issue, copy_out);
     if (n_boundaries_out) *n_boundaries_out = nb_total;
     if (n_chars_out) *n_chars_out = nc_total;
     if (overflow) throw Error(kInvalidArgument, "InvalidArgumentError: out_capacity/states_capacity: too small for the batch");
@@ -1106,37 +1223,12 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
         k.bound_offsets = a.bound_offsets;
         k.n_bound = 0;  // no bit stream on this path
         Scratch::ensure(s.d_st8, s.st8_cap, n + 16);
-        Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * n + 16);
-        Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (n + 1) + 16);
-        Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * n + 16);
-        Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (n / 256 + 4));
         k.status8 = static_cast<uint8_t*>(s.d_st8);
-        k.n_tokens = static_cast<uint32_t*>(s.d_ntok);
-        k.tok_base = static_cast<uint64_t*>(s.d_tokbase);
-        k.tok_local = static_cast<uint32_t*>(s.d_toklocal);
-        k.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+        bind_token_counts(s, k, n);
         cuda_check(launch_compact(k, st), "launch(compact)");
-        Scratch::ensure(s.d_tok, s.tok_cap, 4 * nbytes + 16);
-        Scratch::ensure(s.d_cand, s.cand_cap, nbytes * std::max<size_t>(p.n_tags, 1) + 16);
-        Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * nbytes + 16);
-        TagArgs g;
-        g.text = a.text;
-        g.offsets = a.offsets;
-        g.trims = a.trims;
-        g.n_sent = n;
-        g.status = a.status;
-        g.boundaries = a.boundaries;
-        g.bound_offsets = a.bound_offsets;
-        g.char_offsets = a.char_offsets;
-        g.char_states = p.dt.char_rels ? a.char_states : nullptr;
-        g.type_states = p.dt.type_rels ? a.type_states : nullptr;
+        TagArgs g = tag_args(p.dt, a);
         g.tok_base = k.tok_base;
-        g.tok_ids = static_cast<int32_t*>(s.d_tok);
-        g.tok_cands = static_cast<uint8_t*>(s.d_cand);
-        g.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-        g.max_tokens = nbytes;
-        Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nbytes + 32);
-        g.tok_work = static_cast<uint32_t*>(s.d_tokwork);
+        bind_token_records(p, s, g, nbytes);
         g.norm = normalize ? 1 : 0;
         if ((job.dumps & kDumpTagScores) && sc) *sc = bind_tag_scores(s, nbytes, device_score_len_bound(&p));
         cuda_check(launch_tags(p.dt, g, st, (job.dumps & kDumpTagScores) && sc ? sc : nullptr), "launch(tags)");
@@ -1440,8 +1532,6 @@ const char* gold_error_text(uint32_t kind) {
 // chunk's kernels are queued before the host waits for the oldest.  Chunks retire in order.  The ring knows neither where
 // a chunk's bytes come from nor where tokenised bytes go: the whole-buffer calls submit cuts of the caller's buffer and
 // copy into the caller's output, the stream submits its pinned staging buffers and hands its output to `write`.
-
-constexpr size_t kRingDepth = 4;
 
 struct LineRing {
     struct Slot {
@@ -2211,16 +2301,7 @@ int vpt_predict_batch_tags(const vpt_predictor* p, const uint8_t* utf8, const ui
     cuda_check(launch_batch(p->dm, a, st), "launch(batch)");
     uint32_t* d_unserved = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(s.d_ws) + wl.ticket + 128);
     cuda_check(cudaMemsetAsync(d_unserved, 0, 4, st), "memset");
-    TagArgs t;
-    t.text = a.text;
-    t.offsets = a.offsets;
-    t.n_sent = n_sent;
-    t.status = a.status;
-    t.boundaries = a.boundaries;
-    t.bound_offsets = a.bound_offsets;
-    t.char_offsets = a.char_offsets;
-    t.char_states = p->dt.char_rels ? a.char_states : nullptr;
-    t.type_states = p->dt.type_rels ? a.type_states : nullptr;
+    TagArgs t = tag_args(p->dt, a);
     t.tag_token = static_cast<int32_t*>(s.d_tok);
     t.tag_cand = static_cast<int32_t*>(s.d_cand);
     t.n_unserved = d_unserved;
@@ -2320,43 +2401,17 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
         throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
 
-    // Chunks flow through three host-side stages, each one chunk behind the previous one, so that the device always has
-    // the next chunk's kernels queued while the host waits for a chunk's totals:
-    //   A  copy-in + count pass                         -> boundaries / characters of the chunk (pinned host words)
-    //   B  scoring (+ tag prediction) + compaction      -> the chunk's first boundary bit is known from A's totals
-    //   C  copy-out (bit words, per-sentence words, token records at the running token total)
-    const size_t kChunkSentences = chunk_sentences();
-    const std::vector<size_t> sizes = ramp_schedule(n_sent, kChunkSentences, kChunkSentences / 8, kChunkSentences / 4);
-    const size_t nchunks = sizes.size();
-    constexpr int kDepth = 4;
-    std::unique_ptr<ScratchLease> lease[kDepth];
-    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
-    struct CChunk {
-        ChunkState cs;
-        uint64_t nb = 0, nc = 0, nb_base = 0;
-        cudaEvent_t kernels = nullptr;
-        bool issued = false, copied = false;
-    };
-    std::vector<CChunk> chunks(nchunks);
-    struct EventGuard {
-        std::vector<CChunk>& c;
-        ~EventGuard() { for (auto& x : c) { if (x.cs.counted) cudaEventDestroy(x.cs.counted); if (x.kernels) cudaEventDestroy(x.kernels); x.cs.tr.destroy(); } }
-    } guard{chunks};
-    for (size_t c = 0, lo = 0; c < nchunks; lo += sizes[c], ++c) {
-        ChunkState& ch = chunks[c].cs;
-        ch.s_lo = lo;
-        ch.n = sizes[c];
-        ch.byte_lo = byte_offsets[ch.s_lo];
-        if (byte_offsets[ch.s_lo + ch.n] < ch.byte_lo)
-            throw Error(kInvalidArgument, "InvalidArgumentError: byte_offsets: must be non-decreasing");
-        ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
-    }
+    // Every chunk goes through the batch ring: copy-in + count pass (the boundaries and characters of the chunk), then
+    // scoring (+ tag prediction) + compaction (the chunk's first boundary bit is known from the running total), then,
+    // one chunk behind, the copy-out (bit words, per-sentence words, token records at the running token total).
+    BatchRing ring(*p, "compact", "sync(score)", byte_offsets, sentence_chunks(byte_offsets, n_sent));
+    const size_t nchunks = ring.chunks.size();
     const size_t nt = want_tags ? p->n_tags : 0;
     const size_t score_len = want_scores ? device_score_len_bound(p) : 0;
     uint64_t nb_total = 0, tok_total = 0, unserved_total = 0, score_total = 0;
     bool overflow = false;
     // pinned words that receive every chunk's first bit word (merged into the output at the end)
-    Scratch& s0 = *lease[0]->s;
+    Scratch& s0 = ring.scratch(0);
     if (s0.side_cap < nchunks) {
         if (s0.h_side) { cudaFreeHost(s0.h_side); s0.h_side = nullptr; s0.side_cap = 0; }
         const size_t want = std::max<size_t>(256, 2 * nchunks);
@@ -2365,30 +2420,25 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
     }
     uint32_t* const h_side = s0.h_side;
     std::vector<uint32_t> h_unserved(nchunks, 0);
+    std::vector<uint64_t> nb_base(nchunks, 0);  // the chunk's first boundary in the batch
+    std::vector<char> copied(nchunks, 0);       // the chunk's first bit word is in h_side
 
-    auto stage_b = [&](size_t c) {
-        CChunk& cc = chunks[c];
-        ChunkState& ch = cc.cs;
-        Scratch& s = *lease[c % kDepth]->s;
+    auto issue = [&](size_t c, ChunkState& ch, Scratch& s) {
         cudaStream_t st = s.stream;
-        cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
-        cc.nb = s.h_totals[0];
-        cc.nc = s.h_totals[1];
-        cc.nb_base = nb_total;
-        nb_total += cc.nb;
-        if (!cc.kernels) cuda_check(cudaEventCreateWithFlags(&cc.kernels, cudaEventDisableTiming), "cudaEventCreate");
-        if ((nb_total + 31) / 32 > bits_capacity_words || (nb_total && !boundary_bits_out)) { overflow = true; return; }
+        nb_base[c] = nb_total;
+        nb_total += ch.nb;
+        if ((nb_total + 31) / 32 > bits_capacity_words || (nb_total && !boundary_bits_out)) { overflow = true; return false; }
         BatchArgs& a = ch.a;
-        Scratch::ensure(s.d_bounds, s.bounds_cap, cc.nb + 4);
+        Scratch::ensure(s.d_bounds, s.bounds_cap, ch.nb + 4);
         a.scores = nullptr;
         if (!scores_optional(p->dm)) {
-            Scratch::ensure(s.d_scores, s.scores_cap, 4 * cc.nb + 4);
+            Scratch::ensure(s.d_scores, s.scores_cap, 4 * ch.nb + 4);
             a.scores = static_cast<int32_t*>(s.d_scores);
         }
         a.boundaries = static_cast<uint8_t*>(s.d_bounds);
         if (want_tags) {
-            Scratch::ensure(s.d_cst, s.cst_cap, 4 * cc.nc + 4);
-            Scratch::ensure(s.d_tst, s.tst_cap, 4 * cc.nc + 4);
+            Scratch::ensure(s.d_cst, s.cst_cap, 4 * ch.nc + 4);
+            Scratch::ensure(s.d_tst, s.tst_cap, 4 * ch.nc + 4);
             a.char_states = static_cast<uint32_t*>(s.d_cst);
             a.type_states = static_cast<uint32_t*>(s.d_tst);
         }
@@ -2401,80 +2451,45 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
         k.n_chars = a.n_chars;
         k.boundaries = a.boundaries;
         k.bound_offsets = a.bound_offsets;
-        k.n_bound = cc.nb;
-        k.bit_base = uint32_t(cc.nb_base & 31);
-        const size_t nwords = size_t((k.bit_base + cc.nb + 31) / 32);
+        k.n_bound = ch.nb;
+        k.bit_base = uint32_t(nb_base[c] & 31);
+        const size_t nwords = size_t((k.bit_base + ch.nb + 31) / 32);
         Scratch::ensure(s.d_bits, s.bits_cap, 4 * nwords + 16);
         Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
         k.bits = static_cast<uint32_t*>(s.d_bits);
         k.status8 = static_cast<uint8_t*>(s.d_st8);
         if (want_tokens) {
-            Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * ch.n + 16);
-            Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (ch.n + 1) + 16);
-            k.n_tokens = static_cast<uint32_t*>(s.d_ntok);
-            k.tok_base = static_cast<uint64_t*>(s.d_tokbase);
-            Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * ch.n + 16);
-            Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (ch.n / 256 + 4));
-            k.tok_local = static_cast<uint32_t*>(s.d_toklocal);
-            k.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+            bind_token_counts(s, k, ch.n);
             k.tok_total_host = &s.h_totals[4];
         }
         s.h_totals[4] = 0;
         cuda_check(launch_compact(k, st), "launch(compact)");
         if (want_tags) {
-            // a token has at least one character
-            Scratch::ensure(s.d_tok, s.tok_cap, 4 * cc.nc + 16);
-            Scratch::ensure(s.d_cand, s.cand_cap, cc.nc * std::max<size_t>(nt, 1) + 16);
             uint32_t* d_unserved = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(s.d_ws) + workspace_layout(ch.n).ticket + 128);
             cuda_check(cudaMemsetAsync(d_unserved, 0, 4, st), "memset");
-            TagArgs t;
-            t.text = a.text;
-            t.offsets = a.offsets;
-            t.n_sent = ch.n;
-            t.status = a.status;
-            t.boundaries = a.boundaries;
-            t.bound_offsets = a.bound_offsets;
-            t.char_offsets = a.char_offsets;
-            t.char_states = p->dt.char_rels ? a.char_states : nullptr;
-            t.type_states = p->dt.type_rels ? a.type_states : nullptr;
+            TagArgs t = tag_args(p->dt, a);
             t.n_unserved = d_unserved;
             t.tok_base = k.tok_base;
-            t.tok_ids = static_cast<int32_t*>(s.d_tok);
-            t.tok_cands = static_cast<uint8_t*>(s.d_cand);
-            Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * cc.nc + 16);
-            t.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-            t.max_tokens = cc.nc;
-            Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * cc.nc + 32);
-            t.tok_work = static_cast<uint32_t*>(s.d_tokwork);
-            t.text_base = 0;
+            bind_token_records(*p, s, t, ch.nc);  // a token has at least one character
             if (want_scores) {
-                const TagScoreArgs sc = bind_tag_scores(s, cc.nc, score_len);
+                const TagScoreArgs sc = bind_tag_scores(s, ch.nc, score_len);
                 cuda_check(launch_tags(p->dt, t, st, &sc), "launch(tags)");
             } else {
                 cuda_check(launch_tags(p->dt, t, st), "launch(tags)");
             }
             cuda_check(cudaMemcpyAsync(&h_unserved[c], d_unserved, 4, cudaMemcpyDeviceToHost, st), "D2H(unserved)");
         }
-        if (pipeline_trace()) ch.tr.mark(2, st);
-        cuda_check(cudaEventRecord(cc.kernels, st), "cudaEventRecord");
-        cc.issued = true;
+        return true;
     };
-    auto stage_c = [&](size_t c) {
-        CChunk& cc = chunks[c];
-        ChunkState& ch = cc.cs;
-        Scratch& s = *lease[c % kDepth]->s;
-        if (!cc.issued) return;
-        cuda_check(cudaEventSynchronize(cc.kernels), "sync(kernels)");
+    auto copy_out = [&](size_t c, ChunkState& ch, Scratch& s, cudaStream_t so) {
         const uint64_t ntok = want_tokens ? s.h_totals[4] : 0;
         const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
-        if (want_tags && tok_total + ntok > token_capacity) { overflow = true; cc.issued = false; }
+        if (want_tags && tok_total + ntok > token_capacity) overflow = true;
         if (score_total + nsc > score_capacity) overflow = true;
-        cudaStream_t so = s.stream_out;
-        cuda_check(cudaStreamWaitEvent(so, cc.kernels, 0), "cudaStreamWaitEvent");
         if (!overflow) {
-            const uint32_t bit_base = uint32_t(cc.nb_base & 31);
-            const size_t nwords = size_t((bit_base + cc.nb + 31) / 32);
-            const uint64_t w0 = cc.nb_base >> 5;
+            const uint32_t bit_base = uint32_t(nb_base[c] & 31);
+            const size_t nwords = size_t((bit_base + ch.nb + 31) / 32);
+            const uint64_t w0 = nb_base[c] >> 5;
             if (nwords) {
                 // the chunk's first word may share its low bits with the previous chunk: it comes back through a pinned
                 // word and is merged on the host at the end; the other words go straight to their place
@@ -2493,31 +2508,15 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
             }
             if (nsc)
                 cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
+            copied[c] = ch.nb != 0;
         }
-        cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
-        if (pipeline_trace()) ch.tr.mark(3, so);
-        cc.copied = !overflow && cc.nb != 0;
         tok_total += ntok;
         score_total += nsc;
     };
-    // A runs kDepth - 2 chunks ahead of B, B one chunk ahead of C (a scratch is free again when its chunk's C is done)
-    constexpr size_t kAheadA = kDepth - 2;
-    for (size_t c = 0; c < std::min<size_t>(kAheadA, nchunks); ++c) chunk_count(*lease[c % kDepth]->s, chunks[c].cs, utf8, byte_offsets);
-    for (size_t step = 0; step < nchunks + 1; ++step) {
-        if (step + kAheadA < nchunks) chunk_count(*lease[(step + kAheadA) % kDepth]->s, chunks[step + kAheadA].cs, utf8, byte_offsets);
-        if (step < nchunks) stage_b(step);
-        if (step >= 1) stage_c(step - 1);
-    }
-    for (int i = 0; i < kDepth; ++i)
-        if (lease[i]) {
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(score)");
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
-        }
+    ring.run(utf8, byte_offsets, true, issue, copy_out);
     for (uint32_t u : h_unserved) unserved_total += u;
     for (size_t c = 0; c < nchunks; ++c)
-        if (chunks[c].copied) boundary_bits_out[chunks[c].nb_base >> 5] |= h_side[c];
-    if (pipeline_trace())
-        for (size_t c = 0; c < nchunks; ++c) chunks[c].cs.tr.print("compact", c, chunks[c].cs.n, chunks[0].cs.tr);
+        if (copied[c]) boundary_bits_out[nb_base[c] >> 5] |= h_side[c];
     if (n_boundaries_out) *n_boundaries_out = nb_total;
     if (n_tokens_total_out) *n_tokens_total_out = tok_total;
     if (n_unserved_out) *n_unserved_out = unserved_total;
@@ -2606,23 +2605,13 @@ void launch_span_stage(const vpt_predictor* p, const BatchArgs& a, uint32_t wsco
     cuda_check(launch_span_count(g, st), "launch(span count)");
     if (tr) tr->mark_sub(1, st);  // after the filters and the token counts
     if (b.tok_ids) {
-        TagArgs ta;
-        ta.text = a.text;
-        ta.offsets = a.offsets;
-        ta.n_sent = a.n_sent;
-        ta.status = a.status;
-        ta.boundaries = a.boundaries;
-        ta.bound_offsets = a.bound_offsets;
-        ta.char_offsets = a.char_offsets;
-        ta.char_states = p->dt.char_rels ? a.char_states : nullptr;
-        ta.type_states = p->dt.type_rels ? a.type_states : nullptr;
+        TagArgs ta = tag_args(p->dt, a);
         ta.tok_base = g.tok_base;
         ta.tok_ids = b.tok_ids;
         ta.tok_cands = b.tok_cands;
         ta.tok_desc = b.tok_desc;
         ta.max_tokens = b.max_tokens;
         ta.tok_work = b.tok_work;
-        ta.text_base = 0;
         ta.norm = normalize ? 1 : 0;
         cuda_check(launch_tags(p->dt, ta, st, b.scores), "launch(tags)");
     }
@@ -2672,43 +2661,16 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
     DevModel dm = p->dm;
     dm.kytea_norm = normalize ? 1 : 0;
 
-    // Three host-side stages, as in vpt_predict_batch_compact:
-    //   A  copy-in + count pass                  -> boundaries / characters of the chunk (pinned host words)
-    //   B  scoring, line breaks, post-filters, token counts + prefix, (tags), token ends -> tokens of the chunk (pinned)
-    //   C  copy-out (per-document words, token ends and tag records at the running token total)
-    const std::vector<std::pair<size_t, size_t>> cuts = span_chunks(byte_offsets, n_docs);
-    const size_t nchunks = cuts.size();
-    constexpr int kDepth = 4;
-    std::unique_ptr<ScratchLease> lease[kDepth];
-    for (int i = 0; i < kDepth && size_t(i) < nchunks; ++i) lease[i].reset(new ScratchLease(*p));
-    struct SChunk {
-        ChunkState cs;
-        cudaEvent_t kernels = nullptr;
-        bool issued = false;
-    };
-    std::vector<SChunk> chunks(nchunks);
-    struct EventGuard {
-        std::vector<SChunk>& c;
-        ~EventGuard() { for (auto& x : c) { if (x.cs.counted) cudaEventDestroy(x.cs.counted); if (x.kernels) cudaEventDestroy(x.kernels); x.cs.tr.destroy(); } }
-    } guard{chunks};
-    for (size_t c = 0; c < nchunks; ++c) {
-        ChunkState& ch = chunks[c].cs;
-        ch.s_lo = cuts[c].first;
-        ch.n = cuts[c].second;
-        ch.byte_lo = byte_offsets[ch.s_lo];
-        ch.nbytes = byte_offsets[ch.s_lo + ch.n] - ch.byte_lo;
-    }
+    // Every chunk goes through the batch ring: copy-in + count pass, then scoring, line breaks, post-filters, token
+    // counts + prefix, (tags) and token ends (the chunk's tokens to pinned host memory), then, one chunk behind, the
+    // copy-out (per-document words, token ends and tag records at the running token total).
+    BatchRing ring(*p, "spans", "sync(spans)", byte_offsets, span_chunks(byte_offsets, n_docs));
     uint64_t tok_total = 0, score_total = 0;
     bool overflow = false;
 
-    auto stage_b = [&](size_t c) {
-        SChunk& cc = chunks[c];
-        ChunkState& ch = cc.cs;
-        Scratch& s = *lease[c % kDepth]->s;
+    auto issue = [&](size_t, ChunkState& ch, Scratch& s) {
         cudaStream_t st = s.stream;
-        cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
-        const uint64_t nb = s.h_totals[0], nc = s.h_totals[1];
-        if (!cc.kernels) cuda_check(cudaEventCreateWithFlags(&cc.kernels, cudaEventDisableTiming), "cudaEventCreate");
+        const uint64_t nb = ch.nb, nc = ch.nc;
         BatchArgs& a = ch.a;
         Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
         a.scores = nullptr;
@@ -2724,31 +2686,16 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
             a.type_states = static_cast<uint32_t*>(s.d_tst);
         }
         Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
-        Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * ch.n + 16);
-        Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (ch.n + 1) + 16);
-        Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * ch.n + 16);
-        Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (ch.n / kSpanDocs + 4));
         Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
         SpanStage b;
         b.status8 = static_cast<uint8_t*>(s.d_st8);
-        b.n_tokens = static_cast<uint32_t*>(s.d_ntok);
-        b.tok_base = static_cast<uint64_t*>(s.d_tokbase);
-        b.tok_local = static_cast<uint32_t*>(s.d_toklocal);
-        b.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+        bind_token_counts(s, b, ch.n);
         b.tok_total_host = &s.h_totals[4];
         s.h_totals[4] = 0;
         b.token_ends = static_cast<uint32_t*>(s.d_ends);
         TagScoreArgs sc;
         if (tags) {
-            Scratch::ensure(s.d_tok, s.tok_cap, 4 * nc + 16);
-            Scratch::ensure(s.d_cand, s.cand_cap, nc * std::max<size_t>(nt, 1) + 16);
-            Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * nc + 16);
-            Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * nc + 32);
-            b.tok_ids = static_cast<int32_t*>(s.d_tok);
-            b.tok_cands = static_cast<uint8_t*>(s.d_cand);
-            b.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-            b.tok_work = static_cast<uint32_t*>(s.d_tokwork);
-            b.max_tokens = nc;
+            bind_token_records(*p, s, b, nc);
             if (want_scores) {
                 sc = bind_tag_scores(s, nc, score_len);
                 b.scores = &sc;
@@ -2759,22 +2706,13 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
         cuda_check(launch_score(dm, a, st), "launch(score)");
         if (pipeline_trace()) ch.tr.mark_sub(0, st);  // after the scoring kernel
         launch_span_stage(p, a, wsconst_types, normalize, b, st, pipeline_trace() ? &ch.tr : nullptr);
-        if (pipeline_trace()) ch.tr.mark(2, st);
-        cuda_check(cudaEventRecord(cc.kernels, st), "cudaEventRecord");
-        cc.issued = true;
+        return true;
     };
-    auto stage_c = [&](size_t c) {
-        SChunk& cc = chunks[c];
-        ChunkState& ch = cc.cs;
-        Scratch& s = *lease[c % kDepth]->s;
-        if (!cc.issued) return;
-        cuda_check(cudaEventSynchronize(cc.kernels), "sync(kernels)");
+    auto copy_out = [&](size_t, ChunkState& ch, Scratch& s, cudaStream_t so) {
         const uint64_t ntok = s.h_totals[4];
         const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
         if (tok_total + ntok > token_capacity || (ntok && !token_ends_out)) overflow = true;
         if (score_total + nsc > score_capacity) overflow = true;
-        cudaStream_t so = s.stream_out;
-        cuda_check(cudaStreamWaitEvent(so, cc.kernels, 0), "cudaStreamWaitEvent");
         if (!overflow) {
             cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.d_ntok, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
             cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_st8, ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
@@ -2788,26 +2726,10 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
             if (nsc)
                 cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
         }
-        cuda_check(cudaEventRecord(s.ev_out, so), "cudaEventRecord");
-        if (pipeline_trace()) ch.tr.mark(3, so);
         tok_total += ntok;
         score_total += nsc;
     };
-    // A runs kDepth - 2 chunks ahead of B, B one chunk ahead of C (a scratch is free again when its chunk's C is done)
-    constexpr size_t kAheadA = kDepth - 2;
-    for (size_t c = 0; c < std::min<size_t>(kAheadA, nchunks); ++c) chunk_count(*lease[c % kDepth]->s, chunks[c].cs, utf8, byte_offsets);
-    for (size_t step = 0; step < nchunks + 1; ++step) {
-        if (step + kAheadA < nchunks) chunk_count(*lease[(step + kAheadA) % kDepth]->s, chunks[step + kAheadA].cs, utf8, byte_offsets);
-        if (step < nchunks) stage_b(step);
-        if (step >= 1) stage_c(step - 1);
-    }
-    for (int i = 0; i < kDepth; ++i)
-        if (lease[i]) {
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream), "sync(spans)");
-            cuda_check(cudaStreamSynchronize(lease[i]->s->stream_out), "sync(copy-out)");
-        }
-    if (pipeline_trace())
-        for (size_t c = 0; c < nchunks; ++c) chunks[c].cs.tr.print("spans", c, chunks[c].cs.n, chunks[0].cs.tr);
+    ring.run(utf8, byte_offsets, true, issue, copy_out);
     if (n_tokens_total_out) *n_tokens_total_out = tok_total;
     if (n_scores_total_out) *n_scores_total_out = score_total;
     if (overflow) {
