@@ -632,6 +632,47 @@ int vpt_token_spans_dev(const vpt_predictor* predictor,
                         int32_t* d_token_ids, uint8_t* d_token_cands,
                         void* d_workspace, uint64_t workspace_bytes, void* cuda_stream);
 
+/* ---- Tokenized text of documents already in device memory -----------------------------------------------------------
+ *
+ * The predict CLI's tokenized text (Sentence::write_tokenized_text, sentence.rs:850-886) for documents that already live
+ * on the GPU, written as a device string column: one string per document and int64 Arrow-style offsets.  Document d is
+ * d_utf8[o[d] .. o[d+1]) with the offsets of vpt_token_spans_dev (int32 or int64, o[0] may be > 0, any text alignment).
+ * Its string is write_tokenized_text of the original document after, in order: KyteaFullwidthFilter (unless no_norm),
+ * predict, the wsconst post-filters (as vpt_tokenize_lines, VPT_WSCONST_GRAPHEME included), with predict_tags fill_tags
+ * and, with `rules`, PatternMatchTagger keyed as vpt_tokenize_lines_tags_rules keys it.  '\r' and '\n' are ordinary
+ * characters: there is no line splitting and no terminator, so a document without '\n', followed by "\n", is what
+ * vpt_tokenize_lines writes for it as one line with the same flags.  A document that Sentence::from_raw rejects gets
+ * d_status VPT_SENT_EMPTY / VPT_SENT_NUL / VPT_SENT_BAD_UTF8, one whose offsets are not a range VPT_SENT_BAD_RANGE
+ * (as vpt_token_spans_dev), and an empty string; the others VPT_SENT_OK.
+ *
+ * Contract: the call never synchronises, allocates, creates events or streams, or writes host memory.  All its work is
+ * queued on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream) and it may be captured in a CUDA graph.
+ *
+ *  - Output.  d_out_offsets [n_docs + 1] is always written in full: [0] = 0 and [d+1] - [d] is the length of document d's
+ *    string.  Document d's bytes go to d_out[d_out_offsets[d] ..] if and only if d_out_offsets[d+1] <= out_capacity;
+ *    nothing else in d_out is touched.  out_capacity == 0 (d_out may then be NULL) is an offsets-only sizing pass.
+ *  - vpt_tokenize_dev_out_bound is a bound the host knows: with out_capacity at least this, every document is written.
+ *    It is 3 * n_bytes (surface bytes, at most one '\' per byte, at most one ' ' per character), plus with tags
+ *    n_bytes * (the model's longest "/tag.." suffix + the rules' longest, computed once by vpt_tag_rules_new).
+ *  - d_workspace: vpt_tokenize_dev_workspace_size(predictor, rules, n_docs, n_bytes, predict_tags) bytes of device
+ *    scratch, 256-byte aligned inside.
+ *  - Checked on the host, before anything is queued: NULL pointers, offset_bytes, the workspace size, the flags (as
+ *    vpt_tokenize_lines_tags: VPT_UNSUPPORTED for a tag model beyond the device tables), that `rules` needs predict_tags
+ *    and belongs to the predictor, that every pointer is device memory of the predictor's device, and the batch limit:
+ *    n_bytes and n_docs at most 2^32 - 16, each document at most 1 GiB (a longer one is VPT_SENT_BAD_RANGE).
+ *  - A predictor with predict_tags but no tag slots writes the untagged text, as vpt_tokenize_lines_tags.
+ *  - n_docs == 0 writes d_out_offsets[0] = 0 and returns VPT_OK (d_status and the workspace may then be NULL). */
+uint64_t vpt_tokenize_dev_workspace_size(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
+                                         size_t n_docs, uint64_t n_bytes, int predict_tags);
+uint64_t vpt_tokenize_dev_out_bound(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
+                                    size_t n_docs, uint64_t n_bytes, int predict_tags);
+int vpt_tokenize_dev(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
+                     const uint8_t* d_utf8, uint64_t n_bytes, const void* d_offsets, int offset_bytes, size_t n_docs,
+                     int no_norm, uint32_t wsconst_types, int predict_tags,
+                     int64_t* d_out_offsets /* [n_docs + 1] */, uint8_t* d_out /* nullable if out_capacity == 0 */,
+                     uint64_t out_capacity, uint8_t* d_status /* [n_docs] */,
+                     void* d_workspace, uint64_t workspace_bytes, void* cuda_stream);
+
 /* `KyteaFullwidthFilter` for one character (vaporetto_rules/src/string_filters/kytea_fullwidth.rs:13-118): the
  * same function the kernels apply (csrc/textnorm.hpp). */
 uint32_t vpt_kytea_fullwidth(uint32_t code_point);

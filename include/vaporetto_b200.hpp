@@ -285,6 +285,37 @@ public:
                                           out.token_cands, out.workspace, out.workspace_bytes, stream));
     }
 
+    /// Device buffers of `tokenize_dev` (see `vpt_tokenize_dev` for their sizes)
+    struct DeviceText {
+        int64_t* offsets = nullptr;         // n_documents + 1
+        uint8_t* chars = nullptr;           // capacity bytes; nullable when capacity == 0 (offsets only)
+        uint64_t capacity = 0;
+        uint8_t* status = nullptr;          // n_documents
+        void* workspace = nullptr;          // tokenize_dev_workspace_size bytes
+        uint64_t workspace_bytes = 0;
+    };
+    /// bytes of device scratch `tokenize_dev` needs (vpt_tokenize_dev_workspace_size)
+    uint64_t tokenize_dev_workspace_size(size_t n_docs, uint64_t n_bytes, bool predict_tags = false,
+                                         const TagRules* tag_rules = nullptr) const {
+        return vpt_tokenize_dev_workspace_size(h_, detail::rules_handle(tag_rules), n_docs, n_bytes, predict_tags ? 1 : 0);
+    }
+    /// a capacity of `DeviceText::chars` with which every document is written (vpt_tokenize_dev_out_bound)
+    uint64_t tokenize_dev_out_bound(size_t n_docs, uint64_t n_bytes, bool predict_tags = false,
+                                    const TagRules* tag_rules = nullptr) const {
+        return vpt_tokenize_dev_out_bound(h_, detail::rules_handle(tag_rules), n_docs, n_bytes, predict_tags ? 1 : 0);
+    }
+    /// `tokenize` for documents already in device memory (`vpt_tokenize_dev`): the tokenized text of every document as
+    /// a device string column; `d_offsets` holds n_docs + 1 int32 (offset_bytes 4) or int64 (8) offsets into `d_utf8`.
+    /// All work is queued on `stream` (a cudaStream_t), nothing is synchronised or allocated, so the call can be captured
+    /// in a CUDA graph.  `tag_rules`: PatternMatchTagger after fill_tags (with predict_tags only).
+    void tokenize_dev(const uint8_t* d_utf8, uint64_t n_bytes, const void* d_offsets, int offset_bytes, size_t n_docs,
+                      const DeviceText& out, bool no_norm = false, uint32_t wsconst_types = 0, bool predict_tags = false,
+                      const TagRules* tag_rules = nullptr, void* stream = nullptr) const {
+        detail::check(vpt_tokenize_dev(h_, detail::rules_handle(tag_rules), d_utf8, n_bytes, d_offsets, offset_bytes, n_docs,
+                                       no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0, out.offsets, out.chars,
+                                       out.capacity, out.status, out.workspace, out.workspace_bytes, stream));
+    }
+
     /// the longest tag score vector of the predictor's tokens (vpt_tag_score_len)
     size_t max_score_len() const {
         size_t m = 0;

@@ -14,7 +14,7 @@ import numpy as np
 
 __all__ = ["Model", "Predictor", "Sentence", "VaporettoError", "CharacterBoundary", "CharacterType", "lib", "build",
            "BatchResult", "build_blob", "shard_by_bytes", "LineStream", "SpansResult", "SpanToken", "Tokenizer",
-           "PatternMatchTagger", "DeviceSpans"]
+           "PatternMatchTagger", "DeviceSpans", "DeviceText"]
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("VPT_B200_LIBRARY") or os.path.join(_PKG, "libvaporetto_b200.so")  # (override: A/B builds)
@@ -144,6 +144,10 @@ ABI = [
     ("vpt_token_spans_dev_workspace_size", C.c_uint64, [_P, C.c_size_t, C.c_uint64, C.c_int]),
     ("vpt_token_spans_dev", C.c_int, [_P, _P, C.c_uint64, _P, C.c_int, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P,
                                       _P, _P, C.c_uint64, _P]),
+    ("vpt_tokenize_dev_workspace_size", C.c_uint64, [_P, _P, C.c_size_t, C.c_uint64, C.c_int]),
+    ("vpt_tokenize_dev_out_bound", C.c_uint64, [_P, _P, C.c_size_t, C.c_uint64, C.c_int]),
+    ("vpt_tokenize_dev", C.c_int, [_P, _P, _P, C.c_uint64, _P, C.c_int, C.c_size_t, C.c_int, C.c_uint32, C.c_int, _P, _P,
+                                   C.c_uint64, _P, _P, C.c_uint64, _P]),
 ]
 
 # vpt_stream_write_fn: int (*)(void* ctx, const uint8_t* bytes, size_t n)
@@ -634,6 +638,51 @@ class Predictor:
                                          dp(cands) if nt else None, dp(ws), ws_bytes, st.cuda_stream))
         return DeviceSpans(tok_off, n_tokens, status, ends, ids, cands, st, ws)
 
+    def tokenize_device(self, text, offsets, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
+                        tag_rules: Optional["PatternMatchTagger"] = None, out_capacity: Optional[int] = None,
+                        stream=None) -> "DeviceText":
+        """The tokenized text of documents already in GPU memory (vpt_tokenize_dev), as a device string column: one
+        string per document, what tokenize_lines writes for it as one line without the '\n' ('\r' and '\n' inside a
+        document are ordinary characters).  `text` and `offsets` are as in token_spans_device; `wsconst`, `predict_tags`
+        and `tag_rules` as in tokenize_lines (tag_rules needs predict_tags).  `out_capacity`: bytes of the output buffer
+        (None: vpt_tokenize_dev_out_bound, with which every document is written; 0: offsets only).  The call is queued
+        on `stream` (default: torch.cuda.current_stream()), its workspace and outputs come from torch's caching
+        allocator on that stream, and it neither synchronises nor reads anything back: it is stream-ordered and can be
+        captured in a CUDA graph.  A rejected document has a non-zero status (4: offsets out of range) and an empty
+        string.  See DeviceText."""
+        import torch
+        if not isinstance(text, torch.Tensor) or text.dtype != torch.uint8 or text.dim() != 1 or not text.is_cuda:
+            raise VaporettoError(2, "InvalidArgumentError: text: must be a 1-D torch.uint8 CUDA tensor")
+        if (not isinstance(offsets, torch.Tensor) or offsets.dtype not in (torch.int32, torch.int64) or offsets.dim() != 1
+                or offsets.numel() < 1):
+            raise VaporettoError(2, "InvalidArgumentError: offsets: must be a 1-D int32 or int64 tensor of n_docs + 1")
+        if text.device != offsets.device or text.device.index != self.info["device"]:
+            raise VaporettoError(2, f"InvalidArgumentError: text/offsets: must be on the predictor's device "
+                                    f"cuda:{self.info['device']}")
+        if out_capacity is not None and int(out_capacity) < 0:
+            raise VaporettoError(2, "InvalidArgumentError: out_capacity: must not be negative")
+        mask = _wsconst_mask(wsconst)
+        dev = text.device
+        st = torch.cuda.current_stream(dev) if stream is None else stream
+        n, nb = offsets.numel() - 1, text.numel()
+        rules = None if tag_rules is None else tag_rules._handle()
+        L = lib()
+        cap = L.vpt_tokenize_dev_out_bound(self._h, rules, n, nb, int(predict_tags)) if out_capacity is None \
+            else int(out_capacity)
+        with torch.cuda.stream(st):
+            text, offsets = text.contiguous(), offsets.contiguous()
+            ws_bytes = L.vpt_tokenize_dev_workspace_size(self._h, rules, n, nb, int(predict_tags))
+            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+            out_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            chars = torch.empty(cap, dtype=torch.uint8, device=dev)
+            status = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)[:n]  # (an empty tensor has no pointer)
+            _check(L.vpt_tokenize_dev(self._h, rules, text.data_ptr() if nb else None, nb, offsets.data_ptr(),
+                                      offsets.element_size(), n, int(no_norm), mask, int(predict_tags), out_off.data_ptr(),
+                                      chars.data_ptr() if cap else None, cap, status.data_ptr(), ws.data_ptr(), ws_bytes,
+                                      st.cuda_stream))
+            complete = out_off[-1] <= cap
+        return DeviceText(out_off, chars, status, complete, st, (ws, text, offsets, tag_rules))
+
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
                     scores: bool = False, tag_scores: bool = False) -> "LineStream":
@@ -896,6 +945,36 @@ class DeviceSpans:
                            host(self.token_ends[:k], np.uint32),
                            None if self.token_ids is None else host(self.token_ids[:k], np.int32),
                            None if self.token_cands is None else host(self.token_cands[:k], np.uint8))
+
+
+class DeviceText:
+    """Result of Predictor.tokenize_device, torch tensors on the device, valid once the call's stream reaches them: a
+    string column with `offsets` (int64, n_docs + 1: document d's string is chars[offsets[d]:offsets[d + 1]], the total
+    last), `chars` (uint8, the output capacity), `status` (uint8 per document, VPT_SENT_*; 4 = offsets out of range) and
+    `complete`, a 0-d bool tensor: whether every document was written (offsets[-1] <= capacity).  A document is written
+    in full or not at all; with complete False the offsets are still exact, so they size a second call."""
+
+    def __init__(self, offsets, chars, status, complete, stream, keep):
+        self.offsets, self.chars, self.status, self.complete = offsets, chars, status, complete
+        self.stream = stream
+        self._keep = keep  # (the workspace and the inputs stay alive with the outputs: the queued kernels use them)
+
+    def to_host(self):
+        """Synchronises the stream and returns (chars[:total] as a numpy uint8 array, offsets as int64, status as
+        uint8); raises VaporettoError when the output is incomplete."""
+        self.stream.synchronize()
+        off = self.offsets.cpu().numpy()
+        total = int(off[-1])
+        if total > self.chars.numel():
+            raise VaporettoError(2, f"InvalidArgumentError: out_capacity: {self.chars.numel()} bytes, the tokenized text "
+                                    f"needs {total}")
+        return self.chars[:total].cpu().numpy(), off, self.status.cpu().numpy()
+
+    def strings(self) -> List[str]:
+        """Every document's tokenized text (to_host, decoded)."""
+        chars, off, _ = self.to_host()
+        b = chars.tobytes()
+        return [b[off[d]:off[d + 1]].decode() for d in range(off.size - 1)]
 
 
 class SpanToken:

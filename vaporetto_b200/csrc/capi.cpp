@@ -161,6 +161,7 @@ struct vpt_tag_rules {
     void* d_mem = nullptr;
     DevTagRules dr;
     mutable std::atomic<uint64_t> max_out{0};  // largest device output buffer of a chunk with these rules
+    uint32_t max_suffix = 0;                   // the longest TagRulesHost::suffix: bytes a rule adds behind one token
     ~vpt_tag_rules() {
         if (d_mem) {
             cudaSetDevice(p->device);
@@ -1161,6 +1162,66 @@ void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* bytes) {
 size_t device_score_len_bound(const vpt_predictor* p);
 TagScoreArgs bind_tag_scores(Scratch& s, uint64_t nc, size_t len_bound);
 
+// Buffers of the per-token tag records behind a scoring pass (launch_tag_records)
+struct TagRecords {
+    uint8_t* status8 = nullptr;          // token counts and their prefix, as CompactArgs
+    uint32_t* n_tokens = nullptr;
+    uint64_t* tok_base = nullptr;
+    uint32_t* tok_local = nullptr;
+    uint64_t* tok_blk = nullptr;
+    int32_t* tok_ids = nullptr;          // the records, as TagArgs
+    uint8_t* tok_cands = nullptr;
+    uint4* tok_desc = nullptr;
+    uint32_t* tok_work = nullptr;
+    uint64_t max_tokens = 0;
+    const TagScoreArgs* scores = nullptr;  // nullable: store every record's score vector
+    const vpt_tag_rules* rules = nullptr;  // nullable: PatternMatchTagger
+    unsigned long long* rule_words = nullptr;  // with rules: the matched rules' suffix sum, then 4 bytes per token (+ 8)
+};
+
+// The tag part of the tokenized writers, after the post-filters (fill_tags sees the final boundaries,
+// predict/src/main.rs:157-160): tokens per sentence and their prefix, the tag prediction into per-token records and, with
+// rules, every record's rule id (ra).  Fills the tag fields of `t`.
+void launch_tag_records(const vpt_predictor& p, const BatchArgs& a, bool normalize, const TagRecords& r, TokArgs& t,
+                        TagRuleArgs* ra, cudaStream_t st) {
+    CompactArgs k;
+    k.n_sent = a.n_sent;
+    k.status = a.status;
+    k.n_chars = a.n_chars;
+    k.boundaries = a.boundaries;
+    k.bound_offsets = a.bound_offsets;
+    k.n_bound = 0;  // no bit stream on this path
+    k.status8 = r.status8;
+    k.n_tokens = r.n_tokens;
+    k.tok_base = r.tok_base;
+    k.tok_local = r.tok_local;
+    k.tok_blk = r.tok_blk;
+    cuda_check(launch_compact(k, st), "launch(compact)");
+    TagArgs g = tag_args(p.dt, a);
+    g.tok_base = k.tok_base;
+    g.tok_ids = r.tok_ids;
+    g.tok_cands = r.tok_cands;
+    g.tok_desc = r.tok_desc;
+    g.tok_work = r.tok_work;
+    g.max_tokens = r.max_tokens;
+    g.norm = normalize ? 1 : 0;
+    cuda_check(launch_tags(p.dt, g, st, r.scores), "launch(tags)");
+    if (r.rules && ra) {
+        // the rule id of every token, and the sum of the matched rules' suffix bounds in front of them
+        ra->rules = r.rules->dr;
+        ra->tok_rule = reinterpret_cast<int32_t*>(r.rule_words + 1);
+        cuda_check(launch_rule_lookup(ra->rules, g, const_cast<int32_t*>(ra->tok_rule), r.rule_words, st), "launch(rules)");
+    }
+    t.tok_base = k.tok_base;
+    t.tok_ids = g.tok_ids;
+    t.tok_cands = g.tok_cands;
+    t.n_tags = uint32_t(p.n_tags);
+    t.ts_slot = p.dt.ts_slot;
+    t.ts_cand = p.dt.ts_cand;
+    t.ts_ref = p.dt.ts_ref;
+    t.ts_bytes = p.dt.ts_bytes;
+}
+
 // Scores the sentences of `a` (text, offsets, trims, n_sent set; `nbytes` bounds their bytes), runs the --wsconst
 // post-filters and, with `job.tags`, predicts the tags of every token into per-token records (the post-filters ran
 // first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
@@ -1214,40 +1275,21 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     cuda_check(launch_wsconst(t, a.boundaries, job.wsconst, normalize, st), "launch(wsconst)");
     if (job.wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
     if (tags) {
-        // tokens per sentence and their prefix, then the tag prediction into per-token records
-        CompactArgs k;
-        k.n_sent = n;
-        k.status = a.status;
-        k.n_chars = a.n_chars;
-        k.boundaries = a.boundaries;
-        k.bound_offsets = a.bound_offsets;
-        k.n_bound = 0;  // no bit stream on this path
+        TagRecords r;
         Scratch::ensure(s.d_st8, s.st8_cap, n + 16);
-        k.status8 = static_cast<uint8_t*>(s.d_st8);
-        bind_token_counts(s, k, n);
-        cuda_check(launch_compact(k, st), "launch(compact)");
-        TagArgs g = tag_args(p.dt, a);
-        g.tok_base = k.tok_base;
-        bind_token_records(p, s, g, nbytes);
-        g.norm = normalize ? 1 : 0;
-        if ((job.dumps & kDumpTagScores) && sc) *sc = bind_tag_scores(s, nbytes, device_score_len_bound(&p));
-        cuda_check(launch_tags(p.dt, g, st, (job.dumps & kDumpTagScores) && sc ? sc : nullptr), "launch(tags)");
-        if (job.rules && ra) {
-            // the rule id of every token, and the sum of the matched rules' suffix bounds in front of them
-            Scratch::ensure(s.d_trule, s.trule_cap, 4 * nbytes + 16);
-            ra->rules = job.rules->dr;
-            ra->tok_rule = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(s.d_trule) + 8);
-            cuda_check(launch_rule_lookup(ra->rules, g, const_cast<int32_t*>(ra->tok_rule),
-                                          static_cast<unsigned long long*>(s.d_trule), st), "launch(rules)");
+        r.status8 = static_cast<uint8_t*>(s.d_st8);
+        bind_token_counts(s, r, n);
+        bind_token_records(p, s, r, nbytes);
+        if ((job.dumps & kDumpTagScores) && sc) {
+            *sc = bind_tag_scores(s, nbytes, device_score_len_bound(&p));
+            r.scores = sc;
         }
-        t.tok_base = k.tok_base;
-        t.tok_ids = g.tok_ids;
-        t.tok_cands = g.tok_cands;
-        t.n_tags = uint32_t(p.n_tags);
-        t.ts_slot = p.dt.ts_slot;
-        t.ts_cand = p.dt.ts_cand;
-        t.ts_ref = p.dt.ts_ref;
-        t.ts_bytes = p.dt.ts_bytes;
+        if (job.rules && ra) {
+            Scratch::ensure(s.d_trule, s.trule_cap, 4 * nbytes + 16);
+            r.rules = job.rules;
+            r.rule_words = static_cast<unsigned long long*>(s.d_trule);
+        }
+        launch_tag_records(p, a, normalize, r, t, ra, st);
     }
     return t;
 }
@@ -1773,6 +1815,7 @@ int vpt_tag_rules_new(const vpt_predictor* p, uint64_t n_rules, const uint8_t* s
     d.suffix = reinterpret_cast<const uint32_t*>(base + offs[5]);
     d.mask = t.mask;
     d.max_bytes = t.max_bytes;
+    for (uint32_t x : t.suffix) r->max_suffix = std::max(r->max_suffix, x);
     *out = r.release();
     return kOk;
     VPT_API_END
@@ -2881,6 +2924,192 @@ int vpt_token_spans_dev(const vpt_predictor* p, const uint8_t* d_utf8, uint64_t 
     cuda_check(launch_batch(dm, a, st), "launch(batch)");
     cuda_check(launch_doc_status(da, a.status, st), "launch(doc status)");
     launch_span_stage(p, a, wsconst_types, normalize, b, st, nullptr);
+    return kOk;
+    VPT_API_END
+}
+
+namespace {
+
+// Scratch of vpt_tokenize_dev in the caller's workspace: byte offsets of every buffer; 0 size = not used
+struct TokDevLayout {
+    size_t off, bad, dblk, ws, status, boff, coff, bounds, scores, cst, tst, st8, ntok, tokbase, toklocal, tokblk, tokids,
+        tokcands, tokdesc, tokwork, trule, tokg, total;
+};
+TokDevLayout tokenize_dev_layout(const vpt_predictor* p, uint64_t n_docs, uint64_t n_bytes, bool tags, bool rules) {
+    TokDevLayout l = {};
+    const uint64_t n = n_docs, b = n_bytes;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o = align_up(o + bytes, 256); return at; };
+    l.off = take(8 * (n + 1));
+    l.bad = take(n);
+    l.dblk = take(8 * doc_offsets_blocks(n));
+    l.ws = take(workspace_layout(n).total);
+    l.status = take(4 * n);
+    l.boff = take(8 * (n + 1));
+    l.bounds = take(b + 4);  // (the writers read boundaries as words)
+    l.scores = scores_optional(p->dm) ? 0 : take(4 * b + 4);
+    if (tags) {
+        l.coff = take(8 * (n + 1));
+        l.cst = take(4 * b + 4);
+        l.tst = take(4 * b + 4);
+        // token counts and records: tokens <= characters <= bytes
+        l.st8 = take(n + 16);
+        l.ntok = take(4 * n + 16);
+        l.tokbase = take(8 * (n + 1) + 16);
+        l.toklocal = take(4 * n + 16);
+        l.tokblk = take(8 * (n / kSpanDocs + 4));
+        l.tokids = take(4 * b + 16);
+        l.tokcands = take(b * std::max<size_t>(p->n_tags, 1) + 16);
+        l.tokdesc = take(16 * b + 16);
+        l.tokwork = take(4 * b + 32);
+        l.trule = rules ? take(4 * b + 16) : 0;
+    }
+    l.tokg = take(8 * ((n + kGroup - 1) / kGroup + 2));  // the writer's look-back state words, then its ticket
+    l.total = o + 256;
+    return l;
+}
+
+// Whether vpt_tokenize_dev predicts tags / applies rules for these flags (the checks themselves are the call's)
+bool tokenize_dev_tags(const vpt_predictor* p, int predict_tags) { return predict_tags != 0 && p->n_tags > 0; }
+bool tokenize_dev_rules(const vpt_predictor* p, const vpt_tag_rules* rules, int predict_tags) {
+    return rules && rules->n_rules && tokenize_dev_tags(p, predict_tags);
+}
+
+}  // namespace
+
+uint64_t vpt_tokenize_dev_workspace_size(const vpt_predictor* p, const vpt_tag_rules* rules, size_t n_docs, uint64_t n_bytes,
+                                         int predict_tags) {
+    if (!p || p->device < 0) return 0;
+    return tokenize_dev_layout(p, n_docs, n_bytes, tokenize_dev_tags(p, predict_tags),
+                               tokenize_dev_rules(p, rules, predict_tags)).total;
+}
+
+uint64_t vpt_tokenize_dev_out_bound(const vpt_predictor* p, const vpt_tag_rules* rules, size_t /*n_docs*/, uint64_t n_bytes,
+                                    int predict_tags) {
+    if (!p) return 0;
+    // surface bytes + at most one '\\' per byte + at most one ' ' per character; with tags every token (at most one per
+    // byte) may get the longest "/tag.." suffix of the model and of the rules
+    uint64_t bound = 3 * n_bytes;
+    if (tokenize_dev_tags(p, predict_tags))
+        bound += n_bytes * (uint64_t(p->dt.max_suffix) +
+                            (tokenize_dev_rules(p, rules, predict_tags) ? uint64_t(rules->max_suffix) : 0));
+    return bound;
+}
+
+int vpt_tokenize_dev(const vpt_predictor* p, const vpt_tag_rules* rules, const uint8_t* d_utf8, uint64_t n_bytes,
+                     const void* d_offsets, int offset_bytes, size_t n_docs, int no_norm, uint32_t wsconst_types,
+                     int predict_tags, int64_t* d_out_offsets, uint8_t* d_out, uint64_t out_capacity, uint8_t* d_status,
+                     void* d_workspace, uint64_t workspace_bytes, void* cuda_stream) {
+    VPT_API_BEGIN
+    // Every check reads the arguments only: nothing here synchronises, allocates or touches the device's data
+    const bool tags = check_lines_flags(p, wsconst_types, predict_tags != 0);
+    if (rules && !predict_tags)
+        throw Error(kInvalidArgument, "InvalidArgumentError: rules: need predict_tags (PatternMatchTagger fills predicted tags)");
+    if (rules && rules->p != p) throw Error(kInvalidArgument, "InvalidArgumentError: rules: made for another predictor");
+    const bool with_rules = tags && rules && rules->n_rules;
+    if (offset_bytes != 4 && offset_bytes != 8)
+        throw Error(kInvalidArgument, "InvalidArgumentError: offset_bytes: must be 4 (int32) or 8 (int64)");
+    if (!d_offsets || !d_out_offsets || (n_docs > 0 && !d_status))
+        throw Error(kInvalidArgument, "InvalidArgumentError: device buffers: must not be NULL");
+    if (n_bytes > 0 && !d_utf8) throw Error(kInvalidArgument, "InvalidArgumentError: d_utf8: must not be NULL");
+    if (out_capacity > 0 && !d_out)
+        throw Error(kInvalidArgument, "InvalidArgumentError: d_out: must not be NULL when out_capacity > 0");
+    if (n_bytes > kMaxSpansDevBatch || n_docs > kMaxSpansDevBatch)
+        throw Error(kInvalidArgument, "InvalidArgumentError: n_bytes/n_docs: over the batch limit of 2^32 - 16 (32-bit "
+                                      "character and token indexes of the tag kernels)");
+    const TokDevLayout l = tokenize_dev_layout(p, n_docs, n_bytes, tags, with_rules);
+    if (n_docs > 0 && (!d_workspace || workspace_bytes < l.total))
+        throw Error(kInvalidArgument, "InvalidArgumentError: workspace: too small (vpt_tokenize_dev_workspace_size)");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    if (n_bytes > 0) require_device_ptr(p, d_utf8, "d_utf8");
+    require_device_ptr(p, d_offsets, "d_offsets");
+    require_device_ptr(p, d_out_offsets, "d_out_offsets");
+    if (out_capacity > 0) require_device_ptr(p, d_out, "d_out");
+    if (n_docs > 0) {
+        require_device_ptr(p, d_status, "d_status");
+        require_device_ptr(p, d_workspace, "d_workspace");
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    uint64_t* out_off = reinterpret_cast<uint64_t*>(d_out_offsets);
+    if (n_docs == 0) {
+        cuda_check(cudaMemsetAsync(out_off, 0, 8, st), "memset(out offsets)");
+        return kOk;
+    }
+    uint8_t* w = static_cast<uint8_t*>(d_workspace);
+    const bool normalize = no_norm == 0;
+    DevModel dm = p->dm;
+    dm.kytea_norm = normalize ? 1 : 0;
+
+    // the caller's offsets -> offsets into the text rounded down to 16 bytes, and the documents out of range
+    const uintptr_t text_addr = reinterpret_cast<uintptr_t>(d_utf8);
+    DocArgs da;
+    da.offsets = d_offsets;
+    da.wide = offset_bytes == 8;
+    da.n_docs = n_docs;
+    da.n_bytes = n_bytes;
+    da.shift = uint32_t(text_addr & 15);
+    da.out = reinterpret_cast<uint64_t*>(w + l.off);
+    da.bad = w + l.bad;
+    da.blk = reinterpret_cast<uint64_t*>(w + l.dblk);
+    cuda_check(launch_doc_offsets(da, st), "launch(doc offsets)");
+
+    BatchArgs a;
+    a.text = reinterpret_cast<const uint8_t*>(text_addr & ~uintptr_t(15));
+    a.offsets = da.out;
+    a.n_sent = n_docs;
+    bind_workspace(a, w + l.ws, n_docs);
+    a.status = reinterpret_cast<int32_t*>(w + l.status);
+    a.bound_offsets = reinterpret_cast<uint64_t*>(w + l.boff);
+    a.boundaries = w + l.bounds;
+    a.scores = l.scores ? reinterpret_cast<int32_t*>(w + l.scores) : nullptr;
+    if (tags) {
+        a.char_offsets = reinterpret_cast<uint64_t*>(w + l.coff);
+        a.char_states = reinterpret_cast<uint32_t*>(w + l.cst);
+        a.type_states = reinterpret_cast<uint32_t*>(w + l.tst);
+    }
+    cuda_check(launch_batch(dm, a, st), "launch(batch)");
+    cuda_check(launch_doc_status(da, a.status, st), "launch(doc status)");
+
+    TokArgs t;
+    t.text = a.text;
+    t.offsets = a.offsets;
+    t.n_sent = n_docs;
+    t.status = a.status;
+    t.n_chars = a.n_chars;
+    t.boundaries = a.boundaries;
+    t.bound_offsets = a.bound_offsets;
+    cuda_check(launch_wsconst(t, a.boundaries, wsconst_types, normalize, st), "launch(wsconst)");
+    if (wsconst_types & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
+    TagRuleArgs ra;
+    if (tags) {
+        TagRecords r;
+        r.status8 = w + l.st8;
+        r.n_tokens = reinterpret_cast<uint32_t*>(w + l.ntok);
+        r.tok_base = reinterpret_cast<uint64_t*>(w + l.tokbase);
+        r.tok_local = reinterpret_cast<uint32_t*>(w + l.toklocal);
+        r.tok_blk = reinterpret_cast<uint64_t*>(w + l.tokblk);
+        r.tok_ids = reinterpret_cast<int32_t*>(w + l.tokids);
+        r.tok_cands = w + l.tokcands;
+        r.tok_desc = reinterpret_cast<uint4*>(w + l.tokdesc);
+        r.tok_work = reinterpret_cast<uint32_t*>(w + l.tokwork);
+        r.max_tokens = n_bytes;
+        if (with_rules) {
+            r.rules = rules;
+            r.rule_words = reinterpret_cast<unsigned long long*>(w + l.trule);
+        }
+        launch_tag_records(*p, a, normalize, r, t, &ra, st);
+    }
+    // the column writer; its look-back state and ticket are zeroed by the launch
+    t.tok_state = reinterpret_cast<uint64_t*>(w + l.tokg);
+    t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + (n_docs + kGroup - 1) / kGroup);
+    t.total = out_off + n_docs;
+    t.total_host = nullptr;
+    t.out = d_out;
+    ColOut col;
+    col.offsets = out_off;
+    col.capacity = out_capacity;
+    col.status = d_status;
+    cuda_check(launch_tokenize_column(t, ra, col, st), "launch(tok column)");
     return kOk;
     VPT_API_END
 }

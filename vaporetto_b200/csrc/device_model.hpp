@@ -138,6 +138,13 @@ struct TokArgs {
 };
 // zeroes tok_state[0 .. n_groups] (ticket included), then one pass: lengths, offsets (look-back), output bytes
 cudaError_t launch_tokenize(const TokArgs& t, cudaStream_t stream);
+// The column output of vpt_tokenize_dev (launch_tokenize_column, tag_rules.hpp): one string per sentence without '\n' at
+// TokArgs::out, a rejected sentence writes none; TokArgs::total points at offsets[n_sent]
+struct ColOut {
+    uint64_t* offsets = nullptr;  // [n_sent + 1] out: offsets[s] = output offset of sentence s, the total last
+    uint64_t capacity = 0;        // bytes at TokArgs::out: sentence s is written iff offsets[s + 1] <= capacity
+    uint8_t* status = nullptr;    // [n_sent] out: TokArgs::status as bytes (VPT_SENT_*)
+};
 // KyteaWsConstFilter for the character types in `mask` (bit t = CharacterType t): clears boundaries between two
 // characters of such a type; uses text / offsets / trims / status / n_chars / bound_offsets of `t`
 cudaError_t launch_wsconst(const TokArgs& t, uint8_t* boundaries, uint32_t mask, bool norm, cudaStream_t stream);

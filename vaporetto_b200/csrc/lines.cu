@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include "device_model.hpp"
@@ -34,6 +35,20 @@ __device__ __forceinline__ uint32_t warp_incl_scan_u32(uint32_t v, int lane) {
         if (lane >= d) v += o;
     }
     return v;
+}
+__device__ __forceinline__ uint64_t warp_incl_scan_u64(uint64_t v, int lane) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t o = __shfl_up_sync(kFull, v, d);
+        if (lane >= d) v += o;
+    }
+    return v;
+}
+// (the line writers' 32-bit lengths, the column writers' 64-bit ones)
+template <class Len>
+__device__ __forceinline__ Len warp_incl_scan_len(Len v, int lane) {
+    if constexpr (sizeof(Len) == 8) return warp_incl_scan_u64(v, lane);
+    else return warp_incl_scan_u32(v, lane);
 }
 
 // bit 7 of every byte of x that is zero (exact per byte: no borrow between bytes)
@@ -170,11 +185,18 @@ constexpr int kTokThreads = 256;
 //      over the predecessors' published totals (state word = 2 flag bits | 62 value bits);
 //   3. one warp per sentence writes: every byte of the surface goes to  base + index + (escapes and spaces
 //      before it), preceded by its own ' ' (word boundary before this character) and '\' (escape).
+// kCol: the column output of vpt_tokenize_dev (k_tok_write_col): one string per document, no '\n', a rejected document
+// writes nothing; document d's output offset (group base + exclusive prefix in the group) goes to col.offsets[d], its
+// status to col.status[d], and its bytes are written only when they end within col.capacity.  Lengths, in-group sums and output indexes are 64-bit there
+// (a batch of 1 GiB documents); the line writers' 32-bit ones are safe for the line ring's chunks (kMaxLineChunk).
 constexpr uint64_t kStAgg = 1ull << 62, kStIncl = 2ull << 62, kStMask = (1ull << 62) - 1;
 
-__global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t ngroups) {
+template <bool kCol>
+__device__ __forceinline__ void tok_write(const TokArgs& t, uint64_t ngroups, const ColOut& col) {
+    using Len = std::conditional_t<kCol, uint64_t, uint32_t>;
     __shared__ uint64_t s_off[kGroup + 1], s_bo[kGroup];
-    __shared__ uint32_t s_nch[kGroup], s_len[kGroup], s_excl[kGroup];
+    __shared__ uint32_t s_nch[kGroup];
+    __shared__ Len s_len[kGroup], s_excl[kGroup];
     __shared__ uint8_t s_trim[kGroup], s_bad[kGroup];
     __shared__ uint64_t s_base;
     __shared__ uint32_t s_grp;
@@ -202,10 +224,10 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
 #pragma unroll
     for (int it = 0; it < kPerWarp; ++it) {
         const int i = warp + it * (kTokThreads / 32);
-        uint32_t len = 0;
+        Len len = 0;
         r_lo[it] = 0; r_fl[it] = 0; r_at[it] = 0;
         if (i < ns) {
-            len = 1;  // the '\n'
+            if constexpr (!kCol) len = 1;  // the '\n'
             if (!s_bad[i]) {
                 const uint64_t o0 = s_off[i];
                 const uint64_t a0 = o0 & ~3ull;
@@ -254,7 +276,7 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
                             cnt += __popc(eq_bytes(w, 1u) & inside80(addr, c0, c1));
                         }
                     }
-                    len += (b1 - b0) + __reduce_add_sync(kFull, cnt);
+                    len += Len(b1 - b0) + __reduce_add_sync(kFull, cnt);
                 }
             }
         }
@@ -264,8 +286,8 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
 
     // ---- 2. offsets: scan inside the group, look-back across groups -----------------------------------------
     if (warp == 0) {
-        const uint32_t v0 = s_len[2 * lane], v1 = s_len[2 * lane + 1];
-        const uint32_t iv = warp_incl_scan_u32(v0 + v1, lane);
+        const Len v0 = s_len[2 * lane], v1 = s_len[2 * lane + 1];
+        const Len iv = warp_incl_scan_len<Len>(v0 + v1, lane);
         s_excl[2 * lane] = iv - v0 - v1;
         s_excl[2 * lane + 1] = iv - v1;
         const uint64_t total = __shfl_sync(kFull, iv, 31);
@@ -308,12 +330,21 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
     for (int it = 0; it < kPerWarp; ++it) {
         const int i = warp + it * (kTokThreads / 32);
         if (i >= ns) continue;
-        uint8_t* __restrict__ out = t.out + gout + s_excl[i];
-        if (s_bad[i]) {
-            if (lane == 0) out[0] = 0x0A;
-            continue;
+        if constexpr (kCol) {
+            if (lane == 0) {
+                col.offsets[gbase + i] = gout + s_excl[i];
+                col.status[gbase + i] = uint8_t(t.status[gbase + i]);
+            }
+            if (s_bad[i] || gout + s_excl[i] + s_len[i] > col.capacity) continue;
         }
-        if (lane == 0) out[s_len[i] - 1] = 0x0A;
+        uint8_t* __restrict__ out = t.out + gout + s_excl[i];
+        if constexpr (!kCol) {
+            if (s_bad[i]) {
+                if (lane == 0) out[0] = 0x0A;
+                continue;
+            }
+            if (lane == 0) out[s_len[i] - 1] = 0x0A;
+        }
         const uint64_t o0 = s_off[i];
         const uint64_t a0 = o0 & ~3ull;
         const uint32_t b0 = uint32_t(o0 - a0), b1 = uint32_t(s_off[i + 1] - a0) - s_trim[i];
@@ -334,7 +365,8 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
         }
         const uint8_t* __restrict__ base = t.text + a0;
         const uint8_t* __restrict__ bnd = t.boundaries + s_bo[i];
-        uint32_t chars = 0, extra = 0;  // characters / inserted bytes before this window
+        uint32_t chars = 0;  // characters before this window
+        Len extra = 0;       // inserted bytes before this window
         for (uint32_t w0 = 0; w0 < b1; w0 += 128) {
             const uint32_t addr = w0 + 4u * uint32_t(lane);
             uint32_t lo = 0, in80 = 0;
@@ -360,7 +392,7 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
             const uint32_t esc80 = (eq_bytes(lo, 0x20u) | eq_bytes(lo, 0x2Fu) | eq_bytes(lo, 0x5Cu)) & in80;
             const uint32_t nex = __popc(sp80) + __popc(esc80);
             const uint32_t ex_incl = warp_incl_scan_u32(nex, lane);
-            uint32_t at = (addr - b0) + extra + ex_incl - nex;  // output index of byte 0 of this word (if inside)
+            Len at = Len(addr) - b0 + extra + ex_incl - nex;  // output index of byte 0 of this word (if inside)
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const uint32_t bit = 0x80u << (8 * j);
@@ -375,6 +407,12 @@ __global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t n
             extra += __shfl_sync(kFull, ex_incl, 31);
         }
     }
+}
+
+__global__ void __launch_bounds__(kTokThreads) k_tok_write(TokArgs t, uint64_t ngroups) { tok_write<false>(t, ngroups, ColOut()); }
+// (one resident block per SM as the bound: ptxas then keeps the 64-bit indexes in registers instead of spilling them)
+__global__ void __launch_bounds__(kTokThreads, 1) k_tok_write_col(TokArgs t, uint64_t ngroups, ColOut col) {
+    tok_write<true>(t, ngroups, col);
 }
 
 // ---- tokenised output with tags (the CLI's --predict-tags: main.rs:130-136,159-166 + sentence.rs:850-886) ------------------
@@ -426,16 +464,20 @@ __device__ __forceinline__ void tag_suffix_write(const TokArgs& t, const TagRule
     }
 }
 
-// One sentence by one warp: returns the output length without the '\n'; writes the bytes when kWrite.
-template <bool kWrite, bool kRules>
-__device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, const TagRuleArgs& ra, uint64_t s, uint64_t o0, uint64_t o1, uint32_t trim, uint32_t nch,
+// One sentence by one warp: returns the output length without the '\n'; writes the bytes when kWrite.  Len: the type of
+// the sentence's output indexes (uint64_t for the column writers).
+template <bool kWrite, bool kRules, class Len>
+__device__ __forceinline__ Len tagged_sentence(const TokArgs& t, const TagRuleArgs& ra, uint64_t s, uint64_t o0, uint64_t o1, uint32_t trim, uint32_t nch,
                                                     uint8_t* __restrict__ out, int lane) {
     const uint64_t a0 = o0 & ~3ull;
     const uint32_t b0 = uint32_t(o0 - a0), b1 = uint32_t(o1 - a0) - trim;
     const uint8_t* __restrict__ base = t.text + a0;
     const uint8_t* __restrict__ bnd = t.boundaries + t.bound_offsets[s];
     const uint64_t rec0 = t.tok_base[s];
-    uint32_t chars = 0, extra = 0, toks = 0;  // characters / inserted bytes / tokens that ended before this window
+    // characters / inserted bytes / tokens that ended before this window
+    uint32_t chars = 0;
+    Len extra = 0;
+    uint32_t toks = 0;
     for (uint32_t w0 = 0; w0 < b1; w0 += 128) {
         const uint32_t addr = w0 + 4u * uint32_t(lane);
         uint32_t lo = 0, in80 = 0;
@@ -476,7 +518,7 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, const TagR
         const uint32_t nex = nsp + __popc(esc80) + sl_sum;
         const uint32_t ex_incl = warp_incl_scan_u32(nex, lane);
         if (kWrite) {
-            uint32_t at = (addr - b0) + extra + ex_incl - nex;  // output index of byte 0 of this word (if inside)
+            Len at = Len(addr) - b0 + extra + ex_incl - nex;  // output index of byte 0 of this word (if inside)
             uint64_t rec = rec0 + toks + sp_incl - nsp;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
@@ -498,7 +540,7 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, const TagR
         chars += __shfl_sync(kFull, st_incl, 31);
         toks += __shfl_sync(kFull, sp_incl, 31);
     }
-    uint32_t len = (b1 - b0) + extra;
+    Len len = Len(b1 - b0) + extra;
     if (nch > 0) {
         const uint32_t last = tag_suffix_len<kRules>(t, ra, rec0 + toks);
         if (kWrite && lane == 0) tag_suffix_write<kRules>(t, ra, rec0 + toks, out + len);
@@ -507,12 +549,13 @@ __device__ __forceinline__ uint32_t tagged_sentence(const TokArgs& t, const TagR
     return len;
 }
 
-// (kRules: one resident block per SM is enough for ptxas to keep the merge in registers; min blocks 0 is the bound
-// without a minimum, so the path without rules compiles as before)
-template <bool kRules>
-__global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags(TokArgs t, uint64_t ngroups, TagRuleArgs ra) {
+// kCol: the column output, as tok_write<true>
+template <bool kRules, bool kCol>
+__device__ __forceinline__ void tok_write_tags(const TokArgs& t, uint64_t ngroups, const TagRuleArgs& ra, const ColOut& col) {
+    using Len = std::conditional_t<kCol, uint64_t, uint32_t>;
     __shared__ uint64_t s_off[kGroup + 1];
-    __shared__ uint32_t s_nch[kGroup], s_len[kGroup], s_excl[kGroup];
+    __shared__ uint32_t s_nch[kGroup];
+    __shared__ Len s_len[kGroup], s_excl[kGroup];
     __shared__ uint8_t s_trim[kGroup], s_bad[kGroup];
     __shared__ uint64_t s_base;
     __shared__ uint32_t s_grp;
@@ -533,15 +576,15 @@ __global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags(
     __syncthreads();
     // 1. output bytes per sentence
     for (int i = warp; i < ns; i += kTokThreads / 32) {
-        uint32_t len = 1;  // the '\n'
-        if (!s_bad[i]) len += tagged_sentence<false, kRules>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], nullptr, lane);
+        Len len = kCol ? 0 : 1;  // the '\n'
+        if (!s_bad[i]) len += tagged_sentence<false, kRules, Len>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], nullptr, lane);
         if (lane == 0) s_len[i] = len;
     }
     __syncthreads();
     // 2. offsets: scan inside the group, look-back across groups (as k_tok_write)
     if (warp == 0) {
-        const uint32_t v0 = s_len[2 * lane], v1 = s_len[2 * lane + 1];
-        const uint32_t iv = warp_incl_scan_u32(v0 + v1, lane);
+        const Len v0 = s_len[2 * lane], v1 = s_len[2 * lane + 1];
+        const Len iv = warp_incl_scan_len<Len>(v0 + v1, lane);
         s_excl[2 * lane] = iv - v0 - v1;
         s_excl[2 * lane + 1] = iv - v1;
         const uint64_t total = __shfl_sync(kFull, iv, 31);
@@ -579,10 +622,31 @@ __global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags(
     // 3. write
     const uint64_t gout = s_base;
     for (int i = warp; i < ns; i += kTokThreads / 32) {
+        if constexpr (kCol) {
+            if (lane == 0) {
+                col.offsets[gbase + i] = gout + s_excl[i];
+                col.status[gbase + i] = uint8_t(t.status[gbase + i]);
+            }
+            if (s_bad[i] || gout + s_excl[i] + s_len[i] > col.capacity) continue;
+        }
         uint8_t* __restrict__ out = t.out + gout + s_excl[i];
-        if (lane == 0) out[s_len[i] - 1] = 0x0A;
-        if (!s_bad[i]) tagged_sentence<true, kRules>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], out, lane);
+        if constexpr (!kCol) {
+            if (lane == 0) out[s_len[i] - 1] = 0x0A;
+        }
+        if (!s_bad[i]) tagged_sentence<true, kRules, Len>(t, ra, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], out, lane);
     }
+}
+
+// (kRules: one resident block per SM is enough for ptxas to keep the merge in registers; min blocks 0 is the bound
+// without a minimum, so the path without rules compiles as before)
+template <bool kRules>
+__global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags(TokArgs t, uint64_t ngroups, TagRuleArgs ra) {
+    tok_write_tags<kRules, false>(t, ngroups, ra, ColOut());
+}
+template <bool kRules>
+__global__ void __launch_bounds__(kTokThreads, kRules ? 1 : 0) k_tok_write_tags_col(TokArgs t, uint64_t ngroups, TagRuleArgs ra,
+                                                                                     ColOut col) {
+    tok_write_tags<kRules, true>(t, ngroups, ra, col);
 }
 
 // KyteaWsConstFilter (vaporetto_rules/src/sentence_filters/kytea_wsconst.rs:27-44) for a set of character types —
@@ -806,6 +870,17 @@ cudaError_t launch_tokenize_rules(const TokArgs& t, const TagRuleArgs& ra, cudaS
     if (t.tok_base && ra.tok_rule) k_tok_write_tags<true><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra);
     else if (t.tok_base) k_tok_write_tags<false><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra);
     else k_tok_write<<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tokenize_column(const TokArgs& t, const TagRuleArgs& ra, const ColOut& col, cudaStream_t stream) {
+    if (t.n_sent == 0) return cudaMemsetAsync(col.offsets, 0, 8, stream);
+    const uint64_t ngroups = (t.n_sent + kGroup - 1) / kGroup;
+    cudaError_t e = cudaMemsetAsync(t.tok_state, 0, 8 * (ngroups + 1), stream);
+    if (e != cudaSuccess) return e;
+    if (t.tok_base && ra.tok_rule) k_tok_write_tags_col<true><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra, col);
+    else if (t.tok_base) k_tok_write_tags_col<false><<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, ra, col);
+    else k_tok_write_col<<<unsigned(ngroups), kTokThreads, 0, stream>>>(t, ngroups, col);
     return cudaGetLastError();
 }
 

@@ -62,6 +62,10 @@ cudaError_t launch_rule_lookup(const DevTagRules& r, const TagArgs& a, int32_t* 
 struct TokArgs;
 // launch_tokenize (lines.cu) with rules (ra.tok_rule != nullptr): k_tok_write_tags<true>
 cudaError_t launch_tokenize_rules(const TokArgs& t, const TagRuleArgs& ra, cudaStream_t stream);
+struct ColOut;
+// launch_tokenize_rules writing the column output `col` (device_model.hpp) instead of '\n'-terminated lines:
+// k_tok_write_col, k_tok_write_tags_col<kRules>; with n_sent == 0 it writes col.offsets[0] = 0
+cudaError_t launch_tokenize_column(const TokArgs& t, const TagRuleArgs& ra, const ColOut& col, cudaStream_t stream);
 
 // rule id of a token (its KyteaFullwidthFilter image when norm != 0), or -1: the token table's probe over the rule table
 VPT_HD int32_t rule_lookup(const DevTagRules& r, const uint8_t* __restrict__ bytes, uint32_t len, int norm) {
