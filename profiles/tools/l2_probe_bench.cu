@@ -306,8 +306,9 @@ static float time_ms(F&& launch, int reps) {
     return ms / reps;
 }
 
-// k_fused's probe sequence (probe_slots.py's output) at two shared-memory footprints, with the carve-out each needs:
-// the ratio of the rates is what the L1 the smaller footprint leaves is worth to the probes.
+// k_fused's probe sequence (probe_slots.py's output) at four shared-memory footprints, one per H100 carve-out (228, 196,
+// 164 and 132 KB), with the carve-out each needs: the ratio of the rates is what the L1 the smaller footprint leaves is
+// worth to the probes.
 static void probe_seq_test(const char* path, const char* table, uint32_t* sink, int n_sm) {
     FILE* f = fopen(path, "rb");
     if (!f) { fprintf(stderr, "%s: cannot open\n", path); exit(1); }
@@ -328,7 +329,7 @@ static void probe_seq_test(const char* path, const char* table, uint32_t* sink, 
     CK(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, 0));
     const int iters = 256;
     const double probes = double(n_sm) * 768 * iters * 2;
-    const int smem_kb[] = {217, 177};
+    const int smem_kb[] = {217, 177, 146, 130};
     for (int rep = 0; rep < 3; ++rep) {
         for (int kb : smem_kb) {
             const int smem = kb * 1024;
