@@ -513,6 +513,49 @@ int vpt_line_stream_new_rules(const vpt_predictor* predictor, const vpt_tag_rule
                               uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
                               vpt_line_stream** out);
 
+/* ---- Partially annotated lines: the caller's boundaries stay, the model decides the rest, then tags --------------------
+ *
+ * Every line is in the format of `Sentence::from_partial_annotation` (sentence.rs:516-631, the reference train CLI's
+ * --part corpora): a character, then a marker, then a character, ...: '|' is a word boundary, '-' is not one, ' ' leaves
+ * the boundary to the model; tag fields may follow a marker position after '/', and '\' escapes the next character of a
+ * tag field.  Lines are split as in vpt_tokenize_lines.  For every line:
+ *
+ *   pa = Sentence::from_partial_annotation(line)       // given[i]: NotWordBoundary, WordBoundary or Unknown
+ *   s  = Sentence::from_raw(pa.as_raw_text())          // KyteaFullwidthFilter of it unless no_norm
+ *   predictor.predict(&mut s); the wsconst_types post-filters on s
+ *   for every i with given[i] != Unknown: s.boundaries_mut()[i] = given[i]      // the caller's markers win, last
+ *   with predict_tags: s.fill_tags(), then the PatternMatchTagger `rules` (nullable)
+ *   boundaries and tags onto the raw text; write_tokenized_text; "\n"
+ *
+ * The output has the format and escaping of vpt_tokenize_lines_tags.  Definitions of this library, not of a reference
+ * command:
+ *   - the markers apply after the post-filters: a '|' between two Kanji stays with VPT_WSCONST_KANJI;
+ *   - the tags in the input are parsed and checked as the reference parses them, and dropped: output tags are predicted
+ *     tags and rule tags only (fill_tags resets a sentence's tags, predictor.rs:559-562);
+ *   - an empty line gives an empty output line, so output lines stay aligned with input lines
+ *     (`from_partial_annotation("")` is an error; the predict CLI likewise prints an empty line for a line it cannot read).
+ * A malformed line stops the call, as a bad gold line stops vpt_evaluate_lines, and is named by its 0-based line: the
+ * lowest bad line's first violation in the reference's character loop returns VPT_INVALID_ARGUMENT
+ * "InvalidArgumentError: partial_annotation_text: <reason> (line N)" with the reference's reasons "must not contain
+ * NULL" (a NUL in character position), "contains an invalid boundary character: '<c>'" and "invalid annotation" (the
+ * line ends where a character is expected); a line that is not valid UTF-8 returns VPT_IO_ERROR ("stream did not
+ * contain valid UTF-8 (line N)") before anything else on that line.  Output delivered before an error (the line stream's
+ * `write` calls) is a prefix of the output that ends at a line end.
+ * The parse, scoring, post-filters, markers, tags and writer run on the device.  Flags are checked as in
+ * vpt_tokenize_lines_tags(_rules); `out`, `out_capacity`, *out_len and *n_lines as there (the output of a line is at most
+ * that of its raw text in vpt_tokenize_lines_tags).
+ * Not offered: a device-resident variant, partial-annotation output, keeping the input's tags, and score dumps. */
+int vpt_tokenize_partial_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
+                               const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags,
+                               uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
+
+/* A line stream of vpt_tokenize_partial_lines: the same output, errors and line count, on input fed in pieces, with
+ * the progress, memory and error rules above (a malformed line poisons the stream after the output of the lines before
+ * its chunk was written). */
+int vpt_line_stream_new_partial(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, int no_norm,
+                                uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
+                                vpt_line_stream** out);
+
 /* ---- Score dumps: the predict CLI's --scores and --tag-scores (predict/src/main.rs:66-93, 125-181) ------------------
  *
  * A VPT_STREAM_TOKENIZE line stream (with `rules`, nullable, as vpt_line_stream_new_rules) whose output is, per input

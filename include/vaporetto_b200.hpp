@@ -10,7 +10,8 @@
 //                                           iter_tokens, write_tokenized_text)
 //   vaporetto::CharacterBoundary / CharacterType   sentence.rs:9-29,70-82
 //   vaporetto::VaporettoError   errors.rs:15-38 (thrown as a C++ exception; `Result<_, VaporettoError>`)
-//   vaporetto::LineStream   (this library's own) tokenize_lines / evaluate_lines on input fed in pieces, output to a sink
+//   vaporetto::LineStream   (this library's own) tokenize_lines / evaluate_lines / tokenize_partial_lines on input fed
+//                           in pieces, output to a sink
 // Where the reference panics (fill_tags on a predictor created with predict_tags = false, predictor.rs:547-551)
 // this mirror throws VaporettoError(InvalidArgument).
 #pragma once
@@ -144,6 +145,27 @@ public:
                                                 wsconst_types, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl)
                 : vpt_tokenize_lines(h_, reinterpret_cast<const uint8_t*>(text.data()), text.size(), no_norm ? 1 : 0,
                                      wsconst_types, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl);
+            if (rc != 0 && attempt == 0 && n_out > out.size()) { out.assign(size_t(n_out) + 1, '\0'); continue; }  // long tag strings
+            detail::check(rc);
+            break;
+        }
+        out.resize(size_t(n_out));
+        return out;
+    }
+
+    /// tokenize_lines for partially annotated lines (`vpt_tokenize_partial_lines`, Sentence::from_partial_annotation's
+    /// format): the model predicts the raw text, the post-filters run, then every '|' / '-' of a line overrides the
+    /// boundary it marks; tags (and `tag_rules`) follow with `predict_tags`.  A malformed line throws, naming it.
+    std::string tokenize_partial_lines(const std::string& text, bool no_norm = false, uint32_t wsconst_types = 0,
+                                       bool predict_tags = false, const TagRules* tag_rules = nullptr) const {
+        size_t n_lines = 0;
+        for (char c : text) n_lines += c == '\n';
+        std::string out((predict_tags ? 19 : 3) * text.size() + n_lines + 1, '\0');
+        uint64_t n_out = 0, nl = 0;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            const int rc = vpt_tokenize_partial_lines(h_, detail::rules_handle(tag_rules), reinterpret_cast<const uint8_t*>(text.data()),
+                                                      text.size(), no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0,
+                                                      reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl);
             if (rc != 0 && attempt == 0 && n_out > out.size()) { out.assign(size_t(n_out) + 1, '\0'); continue; }  // long tag strings
             detail::check(rc);
             break;
@@ -504,6 +526,15 @@ inline const vpt_tag_rules* rules_handle(const TagRules* r) { return r ? r->hand
 class LineStream {
 public:
     using Sink = std::function<void(const uint8_t* bytes, size_t n)>;
+    struct PartialLines {};  ///< selects the stream of Predictor::tokenize_partial_lines
+    /// The stream of Predictor::tokenize_partial_lines (`vpt_line_stream_new_partial`).
+    LineStream(const Predictor& predictor, PartialLines, Sink sink, bool no_norm = false, uint32_t wsconst_types = 0,
+               bool predict_tags = false, const TagRules* tag_rules = nullptr)
+        : sink_(std::move(sink)) {
+        detail::check(vpt_line_stream_new_partial(predictor.handle(), detail::rules_handle(tag_rules), no_norm ? 1 : 0,
+                                                  wsconst_types, predict_tags ? 1 : 0,
+                                                  sink_ ? &LineStream::write : nullptr, this, &h_));
+    }
     /// kind: VPT_STREAM_TOKENIZE (`sink` receives the tokenised lines) or VPT_STREAM_EVALUATE (`sink` may be empty).
     /// tag_rules: as in Predictor::tokenize_lines.  dumps: VPT_DUMP_SCORES | VPT_DUMP_TAG_SCORES, the predict CLI's
     /// --scores / --tag-scores behind every token line (VPT_STREAM_TOKENIZE only; vpt_line_stream_new_scores).

@@ -24,7 +24,14 @@ tag_candidates(r) for a batch, Predictor.store_tag_scores(True) + Token.tag_cand
 PatternMatchTagger right after the tag prediction: every tag slot the model left empty for a token whose surface has
 a rule gets the rule's tag.  FILE holds one rule per line, written as one token of the tokenized format
 (Sentence::from_tokenized): `surface/tag1//tag3`, '\' escaping the next character; an empty tag field leaves its slot
-alone.  Unless --no-norm, tokens are matched by their full-width-normalised form, so write full-width surfaces."""
+alone.  Unless --no-norm, tokens are matched by their full-width-normalised form, so write full-width surfaces.
+
+--partial-annotation is an extension as well: stdin holds partially annotated lines in the format of the reference's
+Sentence::from_partial_annotation (the train CLI's --part corpora: '|' a boundary, '-' none, ' ' for the model to
+decide, after every character but the last).  The model predicts the rest, --wsconst runs, then the given markers win;
+tags follow with --predict-tags (input tags are dropped).  An empty line gives an empty line; a malformed line stops the
+command with its 0-based line number (vpt_line_stream_new_partial).  It cannot be combined with --scores or
+--tag-scores."""
 import argparse
 import os
 import select
@@ -100,12 +107,17 @@ def main(argv=None) -> int:
     ap.add_argument("--tag-rules", metavar="FILE",
                     help="Extension (not in the reference CLI): PatternMatchTagger rules, one `surface/tag1//tag3` per "
                          "line, filling the tags the model leaves empty; needs --predict-tags")
+    ap.add_argument("--partial-annotation", action="store_true",
+                    help="Extension: the input lines are partially annotated ('|' boundary, '-' none, ' ' unknown); "
+                         "the given markers are kept, the model decides the rest")
     ap.add_argument("--device", type=int, default=0, help="CUDA device ordinal")
     args = ap.parse_args(argv)
     if args.tag_rules and not args.predict_tags:
         ap.error("--tag-rules needs --predict-tags")
     if args.tag_scores and not args.predict_tags:
         ap.error("--tag-scores needs --predict-tags")
+    if args.partial_annotation and (args.scores or args.tag_scores):
+        ap.error("--partial-annotation cannot be combined with --scores or --tag-scores")
     rules = None
     if args.tag_rules:
         try:
@@ -120,7 +132,7 @@ def main(argv=None) -> int:
     print("Start tokenization", file=sys.stderr)
     inp, out = sys.stdin.buffer, sys.stdout.buffer
     t0 = time.perf_counter()
-    with predictor.line_stream(no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
+    with predictor.line_stream(kind="partial" if args.partial_annotation else "tokenize", no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
                                tag_rules=tagger, scores=args.scores, tag_scores=args.tag_scores) as stream:
         while True:
             data = inp.read1(READ_BYTES)

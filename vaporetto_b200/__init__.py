@@ -133,6 +133,9 @@ ABI = [
                                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("vpt_line_stream_new_rules", C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
     ("vpt_line_stream_new_scores", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, C.c_uint32, _P, _P, C.POINTER(_P)]),
+    ("vpt_tokenize_partial_lines", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, _P, C.c_size_t,
+                                             C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("vpt_line_stream_new_partial", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
     ("vpt_tag_n_slots", C.c_uint32, [_P, C.c_uint32]),
@@ -542,6 +545,31 @@ class Predictor:
         _check(rc)
         return out[: n.value], int(nl.value)
 
+    def tokenize_partial_lines(self, data, out: Optional[np.ndarray] = None, no_norm: bool = False, wsconst: str = "",
+                               predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None):
+        """tokenize_lines for partially annotated lines (vpt_tokenize_partial_lines): every line is in the format of
+        the reference's Sentence::from_partial_annotation ('|' boundary, '-' no boundary, ' ' unknown after every
+        character but the last; tag fields after '/' are checked and dropped).  The model predicts the raw text, the
+        `wsconst` post-filters run, then every '|' / '-' of the line overrides the boundary it marks; with
+        `predict_tags` the tags (and `tag_rules`) follow.  An empty line gives an empty output line; a malformed line
+        raises VaporettoError (InvalidArgument, or IOError for invalid UTF-8) naming the first such line.  Returns
+        (uint8 view of the output lines, number of lines)."""
+        mask = _wsconst_mask(wsconst)
+        t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
+        if out is None:
+            out = np.empty((3 + (16 if predict_tags else 0)) * t.size + int(np.count_nonzero(t == 10)) + 16, np.uint8)
+        n = C.c_uint64()
+        nl = C.c_uint64()
+        rules = tag_rules._handle() if tag_rules is not None else None
+        for _ in range(2):
+            rc = lib().vpt_tokenize_partial_lines(self._h, rules, t.ctypes.data, t.size, int(no_norm), mask,
+                                                  int(predict_tags), out.ctypes.data, out.size, C.byref(n), C.byref(nl))
+            if rc == 2 and predict_tags and n.value > out.size:
+                out = np.empty(n.value + 16, np.uint8)   # long tag strings: the call reported the size it needs
+                continue
+            break
+        _check(rc)
+        return out[: n.value], int(nl.value)
 
     def evaluate_lines(self, data, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
                        per_line: bool = False):
@@ -686,7 +714,8 @@ class Predictor:
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
                     scores: bool = False, tag_scores: bool = False) -> "LineStream":
-        """tokenize_lines (kind="tokenize") or evaluate_lines (kind="evaluate") on input fed in pieces of any size,
+        """tokenize_lines (kind="tokenize"), evaluate_lines (kind="evaluate") or tokenize_partial_lines
+        (kind="partial") on input fed in pieces of any size,
         with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream.  `tag_rules`
         as in tokenize_lines.  `scores` / `tag_scores` (tokenize only; `tag_scores` needs predict_tags and a model with
         tag slots) add the predict CLI's --scores / --tag-scores dumps behind every token line
@@ -704,8 +733,8 @@ class LineStream:
 
     def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool,
                  tag_rules: Optional["PatternMatchTagger"] = None, scores: bool = False, tag_scores: bool = False):
-        if kind not in STREAM_KINDS:
-            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize' or 'evaluate'")
+        if kind not in STREAM_KINDS and kind != "partial":
+            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize', 'evaluate' or 'partial'")
         dumps = (DUMP_SCORES if scores else 0) | (DUMP_TAG_SCORES if tag_scores else 0)
         if dumps and kind != "tokenize":
             raise VaporettoError(2, "InvalidArgumentError: scores, tag_scores: kind='tokenize' only")
@@ -718,7 +747,10 @@ class LineStream:
         self._write = STREAM_WRITE_FN(self._sink)  # (kept alive as long as the stream)
         h = _P()
         rules = tag_rules._handle() if tag_rules is not None else None
-        if dumps:
+        if kind == "partial":
+            _check(lib().vpt_line_stream_new_partial(predictor._h, rules, int(no_norm), mask, int(predict_tags),
+                                                     C.cast(self._write, _P), None, C.byref(h)))
+        elif dumps:
             _check(lib().vpt_line_stream_new_scores(predictor._h, rules, int(no_norm), mask, int(predict_tags), dumps,
                                                     C.cast(self._write, _P), None, C.byref(h)))
         else:

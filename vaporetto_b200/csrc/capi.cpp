@@ -23,6 +23,7 @@
 #include "kernel_plan.hpp"
 #include "line_feed.hpp"
 #include "model.hpp"
+#include "partial_parse.hpp"
 #include "predictor_build.hpp"
 #include "grapheme.hpp"
 #include "tag_rules.hpp"
@@ -83,7 +84,8 @@ struct Scratch {
     // score dumps of the lines path (dump.hpp): the token lines in front of their dumps, the per-line sizes
     void* d_stage = nullptr; size_t stage_cap = 0;
     void* d_dsize = nullptr; size_t dsize_cap = 0;
-    // gold corpus and metrics (vpt_evaluate_lines)
+    // gold corpus and metrics (vpt_evaluate_lines); the partial parse (vpt_tokenize_partial_lines) uses gtext, goff,
+    // gcoff, gbnd (its marker codes) and evtot (its error key)
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
     void* d_gcoff = nullptr; size_t gcoff_cap = 0;
@@ -1127,8 +1129,10 @@ struct LineChunk {
 };
 
 // What a line loop computes: the flags of vpt_tokenize_lines*, vpt_evaluate_lines or vpt_line_stream_new, checked
+constexpr int kJobPartial = 2;  // vpt_tokenize_partial_lines / vpt_line_stream_new_partial (no public stream kind)
+
 struct LineJob {
-    int kind;          // VPT_STREAM_TOKENIZE or VPT_STREAM_EVALUATE
+    int kind;          // VPT_STREAM_TOKENIZE, VPT_STREAM_EVALUATE or kJobPartial
     bool normalize;    // KyteaFullwidthFilter (no_norm == 0)
     uint32_t wsconst;  // post-filters (VPT_WSCONST_*)
     bool tags;         // tags predicted on the device
@@ -1226,9 +1230,10 @@ void launch_tag_records(const vpt_predictor& p, const BatchArgs& a, bool normali
 // post-filters and, with `job.tags`, predicts the tags of every token into per-token records (the post-filters ran
 // first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
 // records; its output fields are left to the caller.  With the score dumps the boundary scores stay in `a.scores` and,
-// for --tag-scores, every record's score vector is stored through `sc`.
+// for --tag-scores, every record's score vector is stored through `sc`.  With `part` (partially annotated lines), the
+// caller's markers replace the boundaries they mark after the post-filters, before the tags.
 TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job,
-                      TagRuleArgs* ra = nullptr, TagScoreArgs* sc = nullptr) {
+                      TagRuleArgs* ra = nullptr, TagScoreArgs* sc = nullptr, PartArgs* part = nullptr) {
     const bool normalize = job.normalize, tags = job.tags;
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
@@ -1274,6 +1279,13 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     t.bound_offsets = a.bound_offsets;
     cuda_check(launch_wsconst(t, a.boundaries, job.wsconst, normalize, st), "launch(wsconst)");
     if (job.wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
+    if (part) {
+        part->status = a.status;
+        part->n_chars = a.n_chars;
+        part->bound_offsets = a.bound_offsets;
+        part->boundaries = a.boundaries;
+        cuda_check(launch_part_apply(*part, st), "launch(part apply)");
+    }
     if (tags) {
         TagRecords r;
         Scratch::ensure(s.d_st8, s.st8_cap, n + 16);
@@ -1448,7 +1460,7 @@ LineJob line_job(const vpt_predictor* p, int kind, int no_norm, uint32_t wsconst
     if (rules && rules->p != p)
         throw Error(kInvalidArgument, "InvalidArgumentError: rules: made for another predictor");
     // (rules act on predicted tags only: without them, or without any rule, the call is the one without rules)
-    if (rules && tags && kind == VPT_STREAM_TOKENIZE && rules->n_rules) j.rules = rules;
+    if (rules && tags && kind != VPT_STREAM_EVALUATE && rules->n_rules) j.rules = rules;
     return j;
 }
 
@@ -1554,6 +1566,81 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     }
 }
 
+// stage 1 of a chunk of partially annotated lines: line offsets, the parse (raw text, markers, error key), count +
+// score + post-filters on the raw text, the caller's markers, tags, the tokenized writer over the raw text; the output
+// size and the error key to pinned host memory
+void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
+    cudaStream_t st = s.stream;
+    const size_t n = split_lines(s, ch);
+    if (!s.h_eval) cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s.h_eval), 8 * (kEvalTotals + 1)), "cudaMallocHost");
+    s.h_totals[3] = 0;
+    s.h_eval[kEvalTotals] = kGoldNoError;
+    if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
+    const size_t ng = (n + kGroup - 1) / kGroup;
+    const size_t nb = ch.nbytes;  // bounds the raw bytes, the characters and the markers of the chunk
+    Scratch::ensure(s.d_gtext, s.gtext_cap, nb + 64);
+    Scratch::ensure(s.d_goff, s.goff_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
+    Scratch::ensure(s.d_gbnd, s.gbnd_cap, nb + 4);
+    Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
+    // as lines_stage1: the raw bytes bound the output of the writer (with tags, the longest suffix per token)
+    const size_t out_need = 3 * nb + n + 4 + (job.tags ? nb * p.dt.max_suffix : 0);
+    Scratch::ensure(s.d_out, s.out_cap, out_need);
+    PartArgs e;
+    e.text = ch.sp.text;
+    e.offsets = ch.sp.offsets;
+    e.trims = ch.sp.trims;
+    e.n_sent = n;
+    e.surface = static_cast<uint8_t*>(s.d_gtext);
+    e.surf_offsets = static_cast<uint64_t*>(s.d_goff);
+    e.char_offsets = static_cast<uint64_t*>(s.d_gcoff);
+    e.given = static_cast<uint8_t*>(s.d_gbnd);
+    e.state = static_cast<uint64_t*>(s.d_tokg);
+    e.ticket = reinterpret_cast<uint32_t*>(e.state + ng);
+    e.err = static_cast<uint64_t*>(s.d_evtot) + kEvalTotals;
+    cuda_check(cudaMemsetAsync(e.err, 0xFF, 8, st), "cudaMemset");
+    cuda_check(launch_part_parse(e, st), "launch(part parse)");
+    BatchArgs a;
+    a.text = e.surface;
+    a.offsets = e.surf_offsets;
+    a.n_sent = n;
+    TagRuleArgs ra;
+    TokArgs t = predict_lines(p, s, ch, a, nb, job, &ra, nullptr, &e);
+    if (ra.tok_rule) {
+        // as lines_stage1: the rules' share of the output is sized from the suffixes the chunk's tokens matched
+        cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
+        cuda_check(cudaStreamSynchronize(st), "sync(rules)");
+        Scratch::ensure(s.d_out, s.out_cap, out_need + size_t(s.h_totals[6]));
+        uint64_t seen = job.rules->max_out.load();
+        while (seen < s.out_cap && !job.rules->max_out.compare_exchange_weak(seen, s.out_cap)) {}
+    }
+    // the look-back words of the parse are free again: the writer's come from the same scratch (its launch zeroes them)
+    t.tok_state = static_cast<uint64_t*>(s.d_tokg);
+    t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
+    t.total = t.tok_state + ng + 1;
+    t.total_host = &s.h_totals[3];
+    t.out = static_cast<uint8_t*>(s.d_out);
+    cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
+    cuda_check(cudaMemcpyAsync(&s.h_eval[kEvalTotals], e.err, 8, cudaMemcpyDeviceToHost, st), "D2H(error key)");
+    if (pipeline_trace()) ch.tr.mark(2, st);
+    cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
+}
+
+// The error of a partially annotated line (partial_parse.hpp) from its key; `line` is the line's first byte in the
+// chunk's input, which the host still holds
+std::string part_error_text(uint32_t kind, const uint8_t* line, uint64_t pos) {
+    switch (kind) {
+        case kPartNul: return "must not contain NULL";
+        case kPartBoundary: {
+            // the character at the position (the line is valid UTF-8: its UTF-8 error would come first)
+            const uint8_t b = line[pos];
+            const size_t len = b < 0x80u ? 1 : b < 0xE0u ? 2 : b < 0xF0u ? 3 : 4;
+            return "contains an invalid boundary character: '" + std::string(reinterpret_cast<const char*>(line + pos), len) + "'";
+        }
+        default: return "invalid annotation";
+    }
+}
+
 const char* gold_error_text(uint32_t kind) {
     switch (kind) {
         case kGoldEmpty: return "must contain at least one character";
@@ -1579,8 +1666,9 @@ struct LineRing {
     struct Slot {
         std::unique_ptr<ScratchLease> lease;
         LineChunk ch;
-        bool stage1 = false;  // lines_stage1 / eval_stage1 issued
+        bool stage1 = false;  // lines_stage1 / eval_stage1 / part_stage1 issued
         size_t index = 0;     // chunk number
+        const uint8_t* input = nullptr;  // the chunk's bytes (untouched until it retires)
     };
     struct Traced {  // trace events of a chunk whose slot was reused before they were printed
         size_t index;
@@ -1634,6 +1722,7 @@ struct LineRing {
         sl.ch.nbytes = n;
         sl.ch.n_lines = 0;
         sl.stage1 = false;
+        sl.input = bytes;
         sl.index = n_chunks++;
         Scratch& s = *sl.lease->s;
         if (trace && sl.index == 0) t0.mark(0, s.stream);
@@ -1646,6 +1735,8 @@ struct LineRing {
         Scratch& s = *sl.lease->s;
         if (job.kind == VPT_STREAM_TOKENIZE) {
             lines_stage1(p, s, sl.ch, job);
+        } else if (job.kind == kJobPartial) {
+            part_stage1(p, s, sl.ch, job);
         } else {
             uint32_t* counts = nullptr;
             if (line_counts) {
@@ -1681,6 +1772,19 @@ struct LineRing {
                                                   " (line " + std::to_string(line) + ")");
             }
             for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
+        } else if (job.kind == kJobPartial) {
+            const uint64_t key = s.h_eval[kEvalTotals];
+            if (key != kGoldNoError) {
+                const uint64_t l = key >> 34;
+                const uint32_t kind = uint32_t(key & 7u);
+                const std::string where = " (line " + std::to_string(lines + l) + ")";
+                if (kind == kPartUtf8) throw Error(kIoError, "stream did not contain valid UTF-8" + where);
+                // the line's first byte: after the l-th '\n' of the chunk
+                const uint8_t* q = sl.input;
+                for (uint64_t k = 0; k < l; ++k) q = static_cast<const uint8_t*>(memchr(q, 0x0A, sl.input + sl.ch.nbytes - q)) + 1;
+                throw Error(kInvalidArgument, "InvalidArgumentError: partial_annotation_text: " +
+                                                  part_error_text(kind, q, ((key >> 3) & 0x7FFFFFFFull) - 1) + where);
+            }
         }
         lines += sl.ch.n_lines;
         ++n_retired;
@@ -1737,15 +1841,15 @@ struct LineRing {
 
 int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
                         uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out,
-                        const vpt_tag_rules* rules = nullptr) {
+                        const vpt_tag_rules* rules = nullptr, int kind = VPT_STREAM_TOKENIZE) {
     VPT_API_BEGIN
-    const LineJob job = line_job(p, VPT_STREAM_TOKENIZE, no_norm, wsconst_types, tags, rules);
+    const LineJob job = line_job(p, kind, no_norm, wsconst_types, tags, rules);
     if (out_len) *out_len = 0;
     if (n_lines_out) *n_lines_out = 0;
     if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     if (n_bytes == 0) return kOk;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-    LineRing ring(*p, job, "lines");
+    LineRing ring(*p, job, kind == kJobPartial ? "partial" : "lines");
     uint64_t total = 0;  // counts on past an overflow: *out_len is the size needed
     bool overflow = false;
     ring.run(utf8, n_bytes, [&](LineRing::Slot& sl) {
@@ -1829,6 +1933,13 @@ int vpt_tokenize_lines_tags_rules(const vpt_predictor* p, const vpt_tag_rules* r
                                   int no_norm, uint32_t wsconst_types, uint8_t* out, size_t out_capacity, uint64_t* out_len,
                                   uint64_t* n_lines_out) {
     return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, true, out, out_capacity, out_len, n_lines_out, rules);
+}
+
+int vpt_tokenize_partial_lines(const vpt_predictor* p, const vpt_tag_rules* rules, const uint8_t* utf8, size_t n_bytes,
+                               int no_norm, uint32_t wsconst_types, int predict_tags, uint8_t* out, size_t out_capacity,
+                               uint64_t* out_len, uint64_t* n_lines_out) {
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, predict_tags != 0, out, out_capacity, out_len,
+                               n_lines_out, rules, kJobPartial);
 }
 
 int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
@@ -1947,7 +2058,7 @@ struct vpt_line_stream {
     // delivers a retired chunk: its output to `write` (tokenize; the ring keeps the evaluate totals)
     void deliver(LineRing::Slot& sl) {
         uint64_t nb = 0;
-        if (ring->job.kind == VPT_STREAM_TOKENIZE) {
+        if (ring->job.kind != VPT_STREAM_EVALUATE) {
             Scratch& s = *sl.lease->s;
             nb = s.h_totals[3];
             if (nb > out.cap) {
@@ -2036,6 +2147,19 @@ int vpt_line_stream_new_scores(const vpt_predictor* p, const vpt_tag_rules* rule
     if ((dumps & VPT_DUMP_TAG_SCORES) && !job.tags)
         throw Error(kInvalidArgument, "InvalidArgumentError: dumps: VPT_DUMP_TAG_SCORES needs a model with tag slots");
     job.dumps = dumps;
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    *out = new vpt_line_stream(p, job, write, ctx);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_line_stream_new_partial(const vpt_predictor* p, const vpt_tag_rules* rules, int no_norm, uint32_t wsconst_types,
+                                int predict_tags, vpt_stream_write_fn write, void* ctx, vpt_line_stream** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    const LineJob job = line_job(p, kJobPartial, no_norm, wsconst_types, predict_tags != 0, rules);
+    if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     *out = new vpt_line_stream(p, job, write, ctx);
     return kOk;

@@ -210,6 +210,34 @@ struct EvalArgs {
 cudaError_t launch_gold_parse(const EvalArgs& e, cudaStream_t stream);
 cudaError_t launch_eval(const EvalArgs& e, cudaStream_t stream);
 
+// ---- partial.cu: partially annotated lines (Sentence::from_partial_annotation, partial_parse.hpp) --------------------
+struct PartArgs {
+    // the chunk's lines (SplitArgs outputs)
+    const uint8_t* text = nullptr;          // readable up to a multiple of 4 past the end
+    const uint64_t* offsets = nullptr;      // [n_sent + 1]
+    const uint8_t* trims = nullptr;         // [n_sent]
+    uint64_t n_sent = 0;
+    // k_part_parse outputs
+    uint8_t* surface = nullptr;             // raw sentence text of every line, concatenated
+    uint64_t* surf_offsets = nullptr;       // [n_sent + 1] into surface
+    uint64_t* char_offsets = nullptr;       // [n_sent + 1] first character of every line
+    uint8_t* given = nullptr;               // [characters + 1] the marker before character k of a line (k >= 1) at
+                                            // char_offsets[line] + k: kPaNot / kPaWord / kPaUnknown
+    uint64_t* state = nullptr;              // [n_groups] look-back scratch
+    uint32_t* ticket = nullptr;             // the 8 bytes after state
+    uint64_t* err = nullptr;                // device scalar: smallest error key line << 34 | (position + 1) << 3 | kind
+                                            // (set to kGoldNoError before the launch)
+    // k_part_apply inputs: the sentences scored on `surface`, after the post-filters
+    const int32_t* status = nullptr;
+    const uint32_t* n_chars = nullptr;
+    const uint64_t* bound_offsets = nullptr;
+    uint8_t* boundaries = nullptr;
+};
+// zeroes state[0 .. n_groups] (ticket included), then parses the lines
+cudaError_t launch_part_parse(const PartArgs& e, cudaStream_t stream);
+// every given '|' / '-' over the boundary it marks
+cudaError_t launch_part_apply(const PartArgs& e, cudaStream_t stream);
+
 // ---- spans.cu: documents -> token byte spans (vaporetto_tantivy's token_stream, vpt_token_spans) --------------------
 struct SpanArgs {
     const uint8_t* text = nullptr;          // as BatchArgs (offsets absolute; readable up to a multiple of 4 past the end)

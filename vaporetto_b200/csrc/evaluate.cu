@@ -13,25 +13,21 @@
 
 #include <cstdint>
 
+#include "byte_window.cuh"
 #include "device_model.hpp"
 
 namespace vpt {
 
 namespace {
 
-constexpr unsigned kFull = 0xFFFFFFFFu;
+using bw::byte_of;
+using bw::inside80;
+using bw::kFull;
+using bw::warp_incl_scan_u32;
+
 constexpr int kEvThreads = 256;
 constexpr int kWarps = kEvThreads / 32;
 constexpr uint64_t kStAgg = 1ull << 62, kStIncl = 2ull << 62, kStMask = (1ull << 62) - 1;
-
-__device__ __forceinline__ uint32_t warp_incl_scan_u32(uint32_t v, int lane) {
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t o = __shfl_up_sync(kFull, v, d);
-        if (lane >= d) v += o;
-    }
-    return v;
-}
 
 // inclusive "last non-zero value" scan: the latest event of a lane or of the lanes before it (0: none)
 __device__ __forceinline__ uint32_t warp_last_scan(uint32_t v, int lane) {
@@ -47,16 +43,6 @@ __device__ __forceinline__ uint32_t zero_bytes(uint32_t x) {
     return ~(((x & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | x) & 0x80808080u;
 }
 __device__ __forceinline__ uint32_t eq_bytes(uint32_t x, uint32_t c) { return zero_bytes(x ^ (c * 0x01010101u)); }
-
-__device__ __forceinline__ uint32_t inside80(uint32_t addr, uint32_t b0, uint32_t b1) {
-    const uint32_t from = b0 > addr ? b0 - addr : 0u;
-    const uint32_t to = b1 - addr < 4u ? b1 - addr : 4u;
-    return (from >= 4u ? 0u : 0x80808080u << (8 * from)) & (0x80808080u >> (8 * (4 - to)));
-}
-
-__device__ __forceinline__ uint32_t byte_of(uint32_t lo, uint32_t hi, int k) {
-    return ((k < 4 ? lo >> (8 * k) : hi >> (8 * (k - 4)))) & 0xFFu;
-}
 
 struct GoldLine {
     uint32_t surf = 0, chars = 0, width = 0;
