@@ -335,6 +335,16 @@ int vpt_write_tokenized_text(const vpt_predictor* predictor, const uint8_t* utf8
                              const uint8_t* boundaries, const int32_t* tag_token, const int32_t* tag_cand,
                              char* buf, size_t capacity, uint64_t* len_out);
 
+/* `Sentence::write_partial_annotation_text` (sentence.rs:907-944): the characters of the text with a marker between each
+ * two ('-' NotWordBoundary, '|' WordBoundary, ' ' Unknown; `boundaries` holds n_chars - 1 values 0 / 1 / 2) and, behind
+ * every character whose tag_cand row has a tag (tag_token/tag_cand as vpt_fill_tags writes them, NULL for none), '/' +
+ * tag for each slot up to the last one that has a tag.  Nothing is escaped, as in the reference: a tag holding ' ', '-',
+ * '|', '/' or '\' does not read back through from_partial_annotation.  Returns the byte length needed in *len_out;
+ * writes at most `capacity` bytes, the last of them a NUL. */
+int vpt_write_partial_annotation_text(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_bytes,
+                                      const uint8_t* boundaries, const int32_t* tag_token, const int32_t* tag_cand,
+                                      char* buf, size_t capacity, uint64_t* len_out);
+
 /* ---- Whole-buffer tokenisation: the reference CLI's loop on the device ----------------------------- */
 
 /* The loop of the reference's `predict` CLI (predict/src/main.rs:126-181) over a whole buffer of raw file bytes:
@@ -544,7 +554,8 @@ int vpt_line_stream_new_rules(const vpt_predictor* predictor, const vpt_tag_rule
  * The parse, scoring, post-filters, markers, tags and writer run on the device.  Flags are checked as in
  * vpt_tokenize_lines_tags(_rules); `out`, `out_capacity`, *out_len and *n_lines as there (the output of a line is at most
  * that of its raw text in vpt_tokenize_lines_tags).
- * Not offered: a device-resident variant, partial-annotation output, keeping the input's tags, and score dumps. */
+ * Not offered: a device-resident variant, keeping the input's tags, and score dumps (partially annotated output is
+ * vpt_annotate_lines). */
 int vpt_tokenize_partial_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
                                const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags,
                                uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
@@ -555,6 +566,44 @@ int vpt_tokenize_partial_lines(const vpt_predictor* predictor, const vpt_tag_rul
 int vpt_line_stream_new_partial(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, int no_norm,
                                 uint32_t wsconst_types, int predict_tags, vpt_stream_write_fn write, void* ctx,
                                 vpt_line_stream** out);
+
+/* ---- Partially annotated output: the boundaries the model is unsure of stay open ----------------------------------------
+ *
+ * The predicted lines in the format of `Sentence::write_partial_annotation_text` (sentence.rs:907-944), with every
+ * boundary whose score lies strictly between -margin and margin left Unknown (' '), for an annotator to resolve before
+ * the corpus goes to the reference's `train --part`.  Lines are split as in vpt_tokenize_lines.  For every line:
+ *
+ *   s = Sentence::from_raw(line)                        // KyteaFullwidthFilter of it unless no_norm
+ *   predictor.predict(&mut s)
+ *   for every boundary i with -margin < score[i] < margin:  s.boundaries_mut()[i] = Unknown      // score: i32
+ *   the wsconst_types post-filters on s                 // they set NotWordBoundary, Unknown or not
+ *   with predict_tags: s.fill_tags(), then the PatternMatchTagger `rules` (nullable)
+ *   boundaries and tags onto the line; write_partial_annotation_text; "\n"
+ *
+ * So:
+ *   - margin 0 leaves nothing Unknown: the output is vpt_tokenize_lines(_tags)'s segmentation in this format;
+ *     a score of exactly +-margin is known, and margin 1 leaves only the scores 0 Unknown;
+ *   - a boundary a post-filter cleared is '-' whatever its score;
+ *   - fill_tags (predictor.rs:567-570) and the rules (iter_tokens, sentence.rs:1273-1299) skip every token next to or
+ *     across an Unknown boundary: such tokens have no tags; every other token has the tags vpt_tokenize_lines_tags(_rules)
+ *     gives it;
+ *   - the characters and the tags are written unescaped, as the reference writes them: a tag that holds ' ', '-', '|',
+ *     '/' or '\' (UniDic-style tags such as "名詞-普通名詞-一般") does not read back through from_partial_annotation;
+ *   - a line update_raw rejects (empty, with a NUL, not valid UTF-8) gives an empty output line.
+ * `margin` must not be negative (VPT_INVALID_ARGUMENT); 0x7FFFFFFF leaves every boundary Unknown that no post-filter
+ * decides except those with the score INT32_MIN.  The scoring, margin, post-filters, tags, rules and writer run on the
+ * device.  Flags are checked as in vpt_tokenize_partial_lines; `out`, `out_capacity`, *out_len and *n_lines as there
+ * (the output of a line is at most that of its text in vpt_tokenize_lines_tags).
+ * Not offered: partially annotated input, a device-resident variant, score dumps, escaped tags. */
+int vpt_annotate_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, const uint8_t* utf8,
+                       size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin, uint8_t* out,
+                       size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
+
+/* A line stream of vpt_annotate_lines: the same output and line count on input fed in pieces, with the progress, memory
+ * and error rules of vpt_line_stream_new_rules. */
+int vpt_line_stream_new_annotate(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, int no_norm,
+                                 uint32_t wsconst_types, int predict_tags, int32_t margin, vpt_stream_write_fn write,
+                                 void* ctx, vpt_line_stream** out);
 
 /* ---- Score dumps: the predict CLI's --scores and --tag-scores (predict/src/main.rs:66-93, 125-181) ------------------
  *

@@ -31,7 +31,13 @@ Sentence::from_partial_annotation (the train CLI's --part corpora: '|' a boundar
 decide, after every character but the last).  The model predicts the rest, --wsconst runs, then the given markers win;
 tags follow with --predict-tags (input tags are dropped).  An empty line gives an empty line; a malformed line stops the
 command with its 0-based line number (vpt_line_stream_new_partial).  It cannot be combined with --scores or
---tag-scores."""
+--tag-scores.
+
+--write-partial-annotation is an extension too: the output lines are in the format of the reference's
+Sentence::write_partial_annotation_text ('|' a boundary, '-' none, ' ' unknown, tags unescaped), and --margin N leaves
+every boundary whose score lies strictly between -N and N unknown for an annotator to resolve (default 0: none); tokens
+next to an unknown boundary get no tags (vpt_line_stream_new_annotate).  It cannot be combined with --scores,
+--tag-scores or --partial-annotation."""
 import argparse
 import os
 import select
@@ -110,6 +116,10 @@ def main(argv=None) -> int:
     ap.add_argument("--partial-annotation", action="store_true",
                     help="Extension: the input lines are partially annotated ('|' boundary, '-' none, ' ' unknown); "
                          "the given markers are kept, the model decides the rest")
+    ap.add_argument("--write-partial-annotation", action="store_true",
+                    help="Extension: write partially annotated lines ('|' boundary, '-' none, ' ' unknown)")
+    ap.add_argument("--margin", type=int, default=0, metavar="N",
+                    help="With --write-partial-annotation: boundaries scoring strictly between -N and N stay unknown")
     ap.add_argument("--device", type=int, default=0, help="CUDA device ordinal")
     args = ap.parse_args(argv)
     if args.tag_rules and not args.predict_tags:
@@ -118,6 +128,12 @@ def main(argv=None) -> int:
         ap.error("--tag-scores needs --predict-tags")
     if args.partial_annotation and (args.scores or args.tag_scores):
         ap.error("--partial-annotation cannot be combined with --scores or --tag-scores")
+    if args.write_partial_annotation and (args.scores or args.tag_scores or args.partial_annotation):
+        ap.error("--write-partial-annotation cannot be combined with --scores, --tag-scores or --partial-annotation")
+    if args.margin and not args.write_partial_annotation:
+        ap.error("--margin needs --write-partial-annotation")
+    if not 0 <= args.margin <= 2**31 - 1:
+        ap.error("--margin must be in 0..2147483647")
     rules = None
     if args.tag_rules:
         try:
@@ -132,8 +148,10 @@ def main(argv=None) -> int:
     print("Start tokenization", file=sys.stderr)
     inp, out = sys.stdin.buffer, sys.stdout.buffer
     t0 = time.perf_counter()
-    with predictor.line_stream(kind="partial" if args.partial_annotation else "tokenize", no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
-                               tag_rules=tagger, scores=args.scores, tag_scores=args.tag_scores) as stream:
+    kind = "partial" if args.partial_annotation else "annotate" if args.write_partial_annotation else "tokenize"
+    with predictor.line_stream(kind=kind, no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
+                               tag_rules=tagger, scores=args.scores, tag_scores=args.tag_scores,
+                               margin=args.margin) as stream:
         while True:
             data = inp.read1(READ_BYTES)
             if not data:

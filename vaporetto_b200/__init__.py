@@ -136,6 +136,10 @@ ABI = [
     ("vpt_tokenize_partial_lines", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, _P, C.c_size_t,
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("vpt_line_stream_new_partial", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, _P, _P, C.POINTER(_P)]),
+    ("vpt_annotate_lines", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, C.c_int32, _P, C.c_size_t,
+                                     C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("vpt_line_stream_new_annotate", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, C.c_int32, _P, _P, C.POINTER(_P)]),
+    ("vpt_write_partial_annotation_text", C.c_int, [_P, _P, C.c_size_t, _P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_uint64)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
     ("vpt_tag_n_slots", C.c_uint32, [_P, C.c_uint32]),
@@ -571,6 +575,31 @@ class Predictor:
         _check(rc)
         return out[: n.value], int(nl.value)
 
+    def annotate_lines(self, data, margin: int = 0, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
+                       tag_rules: Optional["PatternMatchTagger"] = None, out: Optional[np.ndarray] = None):
+        """tokenize_lines in the partial-annotation format (vpt_annotate_lines, the reference's
+        Sentence::write_partial_annotation_text): '|' boundary, '-' no boundary, ' ' Unknown between every two
+        characters.  A boundary whose score lies strictly between -margin and margin is left Unknown, unless a `wsconst`
+        post-filter clears it; tokens next to an Unknown boundary get no tags (`predict_tags`, `tag_rules`).  Tags are
+        written unescaped, as the reference writes them.  margin=0 leaves nothing Unknown.  A line the reference cannot
+        read gives an empty line.  Returns (bytes of the output lines, number of lines)."""
+        mask = _wsconst_mask(wsconst)
+        t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
+        if out is None:
+            out = np.empty((2 + (16 if predict_tags else 0)) * t.size + int(np.count_nonzero(t == 10)) + 16, np.uint8)
+        n = C.c_uint64()
+        nl = C.c_uint64()
+        rules = tag_rules._handle() if tag_rules is not None else None
+        for _ in range(2):
+            rc = lib().vpt_annotate_lines(self._h, rules, t.ctypes.data, t.size, int(no_norm), mask, int(predict_tags),
+                                          int(margin), out.ctypes.data, out.size, C.byref(n), C.byref(nl))
+            if rc == 2 and n.value > out.size:
+                out = np.empty(n.value + 16, np.uint8)   # long tag strings: the call reported the size it needs
+                continue
+            break
+        _check(rc)
+        return out[: n.value].tobytes(), int(nl.value)
+
     def evaluate_lines(self, data, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
                        per_line: bool = False):
         """The reference's `evaluate` command (evaluate/src/main.rs:69-195, vpt_evaluate_lines) over a buffer holding a
@@ -713,14 +742,14 @@ class Predictor:
 
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
-                    scores: bool = False, tag_scores: bool = False) -> "LineStream":
-        """tokenize_lines (kind="tokenize"), evaluate_lines (kind="evaluate") or tokenize_partial_lines
-        (kind="partial") on input fed in pieces of any size,
+                    scores: bool = False, tag_scores: bool = False, margin: int = 0) -> "LineStream":
+        """tokenize_lines (kind="tokenize"), evaluate_lines (kind="evaluate"), tokenize_partial_lines
+        (kind="partial") or annotate_lines (kind="annotate", with `margin`) on input fed in pieces of any size,
         with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream.  `tag_rules`
         as in tokenize_lines.  `scores` / `tag_scores` (tokenize only; `tag_scores` needs predict_tags and a model with
         tag slots) add the predict CLI's --scores / --tag-scores dumps behind every token line
         (vpt_line_stream_new_scores)."""
-        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules, scores, tag_scores)
+        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules, scores, tag_scores, margin)
 
 
 class LineStream:
@@ -732,9 +761,10 @@ class LineStream:
     call close()."""
 
     def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool,
-                 tag_rules: Optional["PatternMatchTagger"] = None, scores: bool = False, tag_scores: bool = False):
-        if kind not in STREAM_KINDS and kind != "partial":
-            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize', 'evaluate' or 'partial'")
+                 tag_rules: Optional["PatternMatchTagger"] = None, scores: bool = False, tag_scores: bool = False,
+                 margin: int = 0):
+        if kind not in STREAM_KINDS and kind not in ("partial", "annotate"):
+            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize', 'evaluate', 'partial' or 'annotate'")
         dumps = (DUMP_SCORES if scores else 0) | (DUMP_TAG_SCORES if tag_scores else 0)
         if dumps and kind != "tokenize":
             raise VaporettoError(2, "InvalidArgumentError: scores, tag_scores: kind='tokenize' only")
@@ -750,6 +780,9 @@ class LineStream:
         if kind == "partial":
             _check(lib().vpt_line_stream_new_partial(predictor._h, rules, int(no_norm), mask, int(predict_tags),
                                                      C.cast(self._write, _P), None, C.byref(h)))
+        elif kind == "annotate":
+            _check(lib().vpt_line_stream_new_annotate(predictor._h, rules, int(no_norm), mask, int(predict_tags),
+                                                      int(margin), C.cast(self._write, _P), None, C.byref(h)))
         elif dumps:
             _check(lib().vpt_line_stream_new_scores(predictor._h, rules, int(no_norm), mask, int(predict_tags), dumps,
                                                     C.cast(self._write, _P), None, C.byref(h)))
@@ -1228,4 +1261,24 @@ class Sentence:
             cap = ln.value + 1
         if ln.value >= cap:
             raise VaporettoError(18, "write_tokenized_text: length changed between calls")
+        return buf.raw[: ln.value].decode("utf-8")
+
+    def write_partial_annotation_text(self) -> str:
+        """`Sentence::write_partial_annotation_text` (sentence.rs:907-944): tags unescaped."""
+        p = self._predictor
+        cap = 2 * len(self._bytes) + 64
+        ln = C.c_uint64()
+        have = self._tags is not None
+        bd = np.ascontiguousarray(self._boundaries, np.uint8)
+        for _ in range(2):
+            buf = C.create_string_buffer(cap)
+            _check(lib().vpt_write_partial_annotation_text(p._h if p else None, self._bytes, len(self._bytes),
+                                                           bd.ctypes.data, self._tag_token.ctypes.data if have else None,
+                                                           self._tag_cand.ctypes.data if have else None, buf, cap,
+                                                           C.byref(ln)))
+            if ln.value < cap:
+                break
+            cap = ln.value + 1
+        if ln.value >= cap:
+            raise VaporettoError(18, "write_partial_annotation_text: length changed between calls")
         return buf.raw[: ln.value].decode("utf-8")

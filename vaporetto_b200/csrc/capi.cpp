@@ -85,7 +85,7 @@ struct Scratch {
     void* d_stage = nullptr; size_t stage_cap = 0;
     void* d_dsize = nullptr; size_t dsize_cap = 0;
     // gold corpus and metrics (vpt_evaluate_lines); the partial parse (vpt_tokenize_partial_lines) uses gtext, goff,
-    // gcoff, gbnd (its marker codes) and evtot (its error key)
+    // gcoff, gbnd (its marker codes) and evtot (its error key); vpt_annotate_lines keeps its output markers in gbnd
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
     void* d_gcoff = nullptr; size_t gcoff_cap = 0;
@@ -1130,15 +1130,17 @@ struct LineChunk {
 
 // What a line loop computes: the flags of vpt_tokenize_lines*, vpt_evaluate_lines or vpt_line_stream_new, checked
 constexpr int kJobPartial = 2;  // vpt_tokenize_partial_lines / vpt_line_stream_new_partial (no public stream kind)
+constexpr int kJobAnnotate = 3;  // vpt_annotate_lines / vpt_line_stream_new_annotate (no public stream kind)
 
 struct LineJob {
-    int kind;          // VPT_STREAM_TOKENIZE, VPT_STREAM_EVALUATE or kJobPartial
+    int kind;          // VPT_STREAM_TOKENIZE, VPT_STREAM_EVALUATE, kJobPartial or kJobAnnotate
     bool normalize;    // KyteaFullwidthFilter (no_norm == 0)
     uint32_t wsconst;  // post-filters (VPT_WSCONST_*)
     bool tags;         // tags predicted on the device
     int tag_mode;      // evaluate: how the system's tags compare with the gold's (kTags*)
     const vpt_tag_rules* rules = nullptr;  // PatternMatchTagger after fill_tags (tokenize with tags and rules only)
     uint32_t dumps = 0;    // tokenize: the predict CLI's --scores / --tag-scores (kDumpScores | kDumpTagScores, dump.hpp)
+    int32_t margin = 0;    // annotate: boundaries with -margin < score < margin are left Unknown
 };
 
 // stage 0 of a chunk: H2D of its `nbytes` at `bytes`, newline counts, the number of lines to pinned host memory
@@ -1231,9 +1233,13 @@ void launch_tag_records(const vpt_predictor& p, const BatchArgs& a, bool normali
 // first: fill_tags sees the final boundaries, predict/src/main.rs:157-160).  Returns the sentences' TokArgs with the tag
 // records; its output fields are left to the caller.  With the score dumps the boundary scores stay in `a.scores` and,
 // for --tag-scores, every record's score vector is stored through `sc`.  With `part` (partially annotated lines), the
-// caller's markers replace the boundaries they mark after the post-filters, before the tags.
+// caller's markers replace the boundaries they mark after the post-filters, before the tags.  With `ann` (partially
+// annotated output, annotate.cu), the boundaries inside `ann->margin` become Unknown before the post-filters; after
+// them every boundary's marker goes to `ann->marks` and the Unknown ones get their predicted value back; the tokens
+// next to an Unknown boundary lose their tag records.
 TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchArgs& a, uint64_t nbytes, const LineJob& job,
-                      TagRuleArgs* ra = nullptr, TagScoreArgs* sc = nullptr, PartArgs* part = nullptr) {
+                      TagRuleArgs* ra = nullptr, TagScoreArgs* sc = nullptr, PartArgs* part = nullptr,
+                      AnnArgs* ann = nullptr) {
     const bool normalize = job.normalize, tags = job.tags;
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
@@ -1249,7 +1255,7 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     a.scores = nullptr;
     DevModel dm = p.dm;
     dm.kytea_norm = normalize ? 1 : 0;
-    if (!scores_optional(dm) || (job.dumps & kDumpScores)) {
+    if (!scores_optional(dm) || (job.dumps & kDumpScores) || (ann && ann->margin > 0)) {
         Scratch::ensure(s.d_scores, s.scores_cap, 4 * nbytes + 4);
         a.scores = static_cast<int32_t*>(s.d_scores);
     }
@@ -1277,6 +1283,15 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     t.n_chars = a.n_chars;
     t.boundaries = a.boundaries;
     t.bound_offsets = a.bound_offsets;
+    if (ann) {
+        ann->n_sent = n;
+        ann->status = a.status;
+        ann->n_chars = a.n_chars;
+        ann->bound_offsets = a.bound_offsets;
+        ann->scores = a.scores;
+        ann->boundaries = a.boundaries;
+        cuda_check(launch_pa_margin(*ann, st), "launch(margin)");
+    }
     cuda_check(launch_wsconst(t, a.boundaries, job.wsconst, normalize, st), "launch(wsconst)");
     if (job.wsconst & 0x80u) cuda_check(launch_grapheme(t, a.boundaries, normalize, st), "launch(grapheme)");
     if (part) {
@@ -1286,6 +1301,7 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
         part->boundaries = a.boundaries;
         cuda_check(launch_part_apply(*part, st), "launch(part apply)");
     }
+    if (ann) cuda_check(launch_pa_marks(*ann, st), "launch(marks)");
     if (tags) {
         TagRecords r;
         Scratch::ensure(s.d_st8, s.st8_cap, n + 16);
@@ -1302,6 +1318,12 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
             r.rule_words = static_cast<unsigned long long*>(s.d_trule);
         }
         launch_tag_records(p, a, normalize, r, t, ra, st);
+        if (ann) {
+            ann->tok_base = t.tok_base;
+            ann->tok_ids = const_cast<int32_t*>(t.tok_ids);
+            ann->tok_rule = ra ? const_cast<int32_t*>(ra->tok_rule) : nullptr;
+            cuda_check(launch_pa_untag(*ann, st), "launch(untag)");
+        }
     }
     return t;
 }
@@ -1399,9 +1421,17 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     void*& tok_buf = job.dumps ? s.d_stage : s.d_out;
     size_t& tok_cap = job.dumps ? s.stage_cap : s.out_cap;
     // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
-    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model)
+    // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model; the
+    // partial-annotation format has one marker per character and no escapes, so the same bound holds for it)
     const size_t out_need = 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0);
     Scratch::ensure(tok_buf, tok_cap, out_need);
+    const bool annotate = job.kind == kJobAnnotate;
+    AnnArgs ann;
+    if (annotate) {
+        Scratch::ensure(s.d_gbnd, s.gbnd_cap, ch.nbytes + 4);
+        ann.margin = job.margin;
+        ann.marks = static_cast<uint8_t*>(s.d_gbnd);
+    }
     BatchArgs a;
     a.text = ch.sp.text;
     a.offsets = ch.sp.offsets;
@@ -1409,7 +1439,7 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     a.n_sent = n;
     TagRuleArgs ra;
     TagScoreArgs sc;
-    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job, &ra, &sc);
+    TokArgs t = predict_lines(p, s, ch, a, ch.nbytes, job, &ra, &sc, nullptr, annotate ? &ann : nullptr);
     if (ra.tok_rule) {
         // A rule's tag may be long on a short surface, so the rules' share of the output is sized from the suffixes the
         // chunk's tokens actually matched: the host waits for the rule lookup and reads their sum.
@@ -1424,7 +1454,8 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     t.total = t.tok_state + ng + 1;
     t.total_host = &s.h_totals[job.dumps ? 4 : 3];
     t.out = static_cast<uint8_t*>(tok_buf);
-    cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
+    if (annotate) cuda_check(launch_pa_write(t, ra, ann.marks, st), "launch(annotate)");
+    else cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
     if (job.dumps) dump_stage(p, s, t, a, sc, ra, job);
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
@@ -1733,7 +1764,7 @@ struct LineRing {
 
     void issue(Slot& sl) {
         Scratch& s = *sl.lease->s;
-        if (job.kind == VPT_STREAM_TOKENIZE) {
+        if (job.kind == VPT_STREAM_TOKENIZE || job.kind == kJobAnnotate) {
             lines_stage1(p, s, sl.ch, job);
         } else if (job.kind == kJobPartial) {
             part_stage1(p, s, sl.ch, job);
@@ -1841,15 +1872,16 @@ struct LineRing {
 
 int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
                         uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out,
-                        const vpt_tag_rules* rules = nullptr, int kind = VPT_STREAM_TOKENIZE) {
+                        const vpt_tag_rules* rules = nullptr, int kind = VPT_STREAM_TOKENIZE, int32_t margin = 0) {
     VPT_API_BEGIN
-    const LineJob job = line_job(p, kind, no_norm, wsconst_types, tags, rules);
+    LineJob job = line_job(p, kind, no_norm, wsconst_types, tags, rules);
+    job.margin = margin;
     if (out_len) *out_len = 0;
     if (n_lines_out) *n_lines_out = 0;
     if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     if (n_bytes == 0) return kOk;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-    LineRing ring(*p, job, kind == kJobPartial ? "partial" : "lines");
+    LineRing ring(*p, job, kind == kJobPartial ? "partial" : kind == kJobAnnotate ? "annotate" : "lines");
     uint64_t total = 0;  // counts on past an overflow: *out_len is the size needed
     bool overflow = false;
     ring.run(utf8, n_bytes, [&](LineRing::Slot& sl) {
@@ -1940,6 +1972,18 @@ int vpt_tokenize_partial_lines(const vpt_predictor* p, const vpt_tag_rules* rule
                                uint64_t* out_len, uint64_t* n_lines_out) {
     return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, predict_tags != 0, out, out_capacity, out_len,
                                n_lines_out, rules, kJobPartial);
+}
+
+int vpt_annotate_lines(const vpt_predictor* p, const vpt_tag_rules* rules, const uint8_t* utf8, size_t n_bytes,
+                       int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin, uint8_t* out,
+                       size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    if (margin < 0) {
+        if (out_len) *out_len = 0;
+        if (n_lines_out) *n_lines_out = 0;
+        return fail(Error(kInvalidArgument, "InvalidArgumentError: margin: must not be negative"));
+    }
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, predict_tags != 0, out, out_capacity, out_len,
+                               n_lines_out, rules, kJobAnnotate, margin);
 }
 
 int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
@@ -2159,6 +2203,22 @@ int vpt_line_stream_new_partial(const vpt_predictor* p, const vpt_tag_rules* rul
     if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
     *out = nullptr;
     const LineJob job = line_job(p, kJobPartial, no_norm, wsconst_types, predict_tags != 0, rules);
+    if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    *out = new vpt_line_stream(p, job, write, ctx);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_line_stream_new_annotate(const vpt_predictor* p, const vpt_tag_rules* rules, int no_norm, uint32_t wsconst_types,
+                                 int predict_tags, int32_t margin, vpt_stream_write_fn write, void* ctx,
+                                 vpt_line_stream** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    LineJob job = line_job(p, kJobAnnotate, no_norm, wsconst_types, predict_tags != 0, rules);
+    if (margin < 0) throw Error(kInvalidArgument, "InvalidArgumentError: margin: must not be negative");
+    job.margin = margin;
     if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     *out = new vpt_line_stream(p, job, write, ctx);
@@ -3362,6 +3422,44 @@ int vpt_write_tokenized_text(const vpt_predictor* p, const uint8_t* utf8, size_t
         } else if (b == 2) skip = true;
     }
     if (!skip) emit(start, n);
+    if (len_out) *len_out = out.size();
+    if (buf && capacity) {
+        const size_t m = std::min(capacity - 1, out.size());
+        memcpy(buf, out.data(), m);
+        buf[m] = 0;
+    }
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_write_partial_annotation_text(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, const uint8_t* boundaries,
+                                      const int32_t* tag_token, const int32_t* tag_cand, char* buf, size_t capacity,
+                                      uint64_t* len_out) {
+    VPT_API_BEGIN
+    if (!utf8 || !boundaries) throw Error(kInvalidArgument, "InvalidArgumentError: utf8/boundaries: must not be NULL");
+    check_raw_text(utf8, n_bytes);
+    const std::vector<uint32_t> pos = char_starts(utf8, n_bytes);
+    const size_t n = pos.size() - 1;
+    const size_t nt = (p && tag_token && tag_cand) ? p->n_tags : 0;
+    std::string out;
+    for (size_t i = 0; i < n; ++i) {
+        if (i > 0) {
+            const uint8_t b = boundaries[i - 1];
+            out.push_back(b == 0 ? '-' : b == 1 ? '|' : ' ');
+        }
+        out.append(reinterpret_cast<const char*>(utf8) + pos[i], pos[i + 1] - pos[i]);
+        // the tags of character i, unescaped, up to the last slot that has one (sentence.rs:907-944)
+        int last = -1;
+        for (size_t k = 0; k < nt; ++k) if (tag_cand[i * nt + k] >= 0) last = int(k);
+        for (int k = 0; k <= last; ++k) {
+            out.push_back('/');
+            const int32_t c = tag_cand[i * nt + size_t(k)];
+            if (c >= 0) {
+                const char* t = vpt_tag_string(p, uint32_t(tag_token[i]), uint32_t(k), uint32_t(c));
+                if (t) out.append(t);
+            }
+        }
+    }
     if (len_out) *len_out = out.size();
     if (buf && capacity) {
         const size_t m = std::min(capacity - 1, out.size());

@@ -238,6 +238,33 @@ cudaError_t launch_part_parse(const PartArgs& e, cudaStream_t stream);
 // every given '|' / '-' over the boundary it marks
 cudaError_t launch_part_apply(const PartArgs& e, cudaStream_t stream);
 
+// ---- annotate.cu: partially annotated output (Sentence::write_partial_annotation_text, vpt_annotate_lines) ------------
+struct AnnArgs {
+    int32_t margin = 0;                     // boundaries with -margin < score < margin become Unknown (0: none)
+    // the scored sentences (BatchArgs outputs)
+    uint64_t n_sent = 0;
+    const int32_t* status = nullptr;
+    const uint32_t* n_chars = nullptr;
+    const uint64_t* bound_offsets = nullptr;
+    const int32_t* scores = nullptr;        // with margin > 0
+    uint8_t* boundaries = nullptr;
+    uint8_t* marks = nullptr;               // [boundaries] out: '-', '|' or ' ' per boundary
+    // k_pa_untag: the tag records (launch_tag_records)
+    const uint64_t* tok_base = nullptr;
+    int32_t* tok_ids = nullptr;
+    int32_t* tok_rule = nullptr;            // nullable: the rule id of every record
+};
+// boundary byte 2 (Unknown) for the scores inside the margin; nothing when margin == 0
+cudaError_t launch_pa_margin(const AnnArgs& a, cudaStream_t stream);
+// the marker of every boundary into marks, and the predicted boundary (score > 0) back into every Unknown one
+cudaError_t launch_pa_marks(const AnnArgs& a, cudaStream_t stream);
+// tok_ids (and tok_rule) = -1 for every token record next to or across a ' ' marker; nothing when margin == 0
+cudaError_t launch_pa_untag(const AnnArgs& a, cudaStream_t stream);
+struct TagRuleArgs;
+// launch_tokenize_rules in the partial-annotation format: the markers from `marks`, the tags of TokArgs (tok_base
+// non-null) and of the rules (ra.tok_rule non-null) unescaped; zeroes tok_state[0 .. n_groups] (ticket included)
+cudaError_t launch_pa_write(const TokArgs& t, const TagRuleArgs& ra, const uint8_t* marks, cudaStream_t stream);
+
 // ---- spans.cu: documents -> token byte spans (vaporetto_tantivy's token_stream, vpt_token_spans) --------------------
 struct SpanArgs {
     const uint8_t* text = nullptr;          // as BatchArgs (offsets absolute; readable up to a multiple of 4 past the end)
