@@ -555,7 +555,7 @@ int vpt_line_stream_new_rules(const vpt_predictor* predictor, const vpt_tag_rule
  * vpt_tokenize_lines_tags(_rules); `out`, `out_capacity`, *out_len and *n_lines as there (the output of a line is at most
  * that of its raw text in vpt_tokenize_lines_tags).
  * Not offered: a device-resident variant, keeping the input's tags, and score dumps (partially annotated output is
- * vpt_annotate_lines). */
+ * vpt_annotate_lines; partially annotated output that keeps the input's markers and tags is vpt_reannotate_lines). */
 int vpt_tokenize_partial_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
                                const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags,
                                uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
@@ -594,7 +594,8 @@ int vpt_line_stream_new_partial(const vpt_predictor* predictor, const vpt_tag_ru
  * decides except those with the score INT32_MIN.  The scoring, margin, post-filters, tags, rules and writer run on the
  * device.  Flags are checked as in vpt_tokenize_partial_lines; `out`, `out_capacity`, *out_len and *n_lines as there
  * (the output of a line is at most that of its text in vpt_tokenize_lines_tags).
- * Not offered: partially annotated input, a device-resident variant, score dumps, escaped tags. */
+ * Not offered: a device-resident variant, score dumps, escaped tags (partially annotated input is
+ * vpt_reannotate_lines). */
 int vpt_annotate_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, const uint8_t* utf8,
                        size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin, uint8_t* out,
                        size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
@@ -604,6 +605,55 @@ int vpt_annotate_lines(const vpt_predictor* predictor, const vpt_tag_rules* rule
 int vpt_line_stream_new_annotate(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, int no_norm,
                                  uint32_t wsconst_types, int predict_tags, int32_t margin, vpt_stream_write_fn write,
                                  void* ctx, vpt_line_stream** out);
+
+/* ---- Re-annotation: partially annotated lines in, partially annotated lines out ---------------------------------------
+ *
+ * The second round of the domain-adaptation loop: a corpus that an annotator has partly resolved (vpt_annotate_lines'
+ * output with some ' ' turned into '|' or '-' and some tags fixed) goes through a retrained model.  Every decision in the
+ * input stays as written; only the positions still undecided are predicted, and those the model is unsure of stay open.
+ * Lines are split as in vpt_tokenize_lines.  For every line:
+ *
+ *   pa = Sentence::from_partial_annotation(line)      // given[i] in {Not, Word, Unknown}; input tag fields per character
+ *   s  = Sentence::from_raw(pa.as_raw_text())          // KyteaFullwidthFilter of it unless no_norm
+ *   predictor.predict(&mut s)
+ *   for every i with -margin < score[i] < margin: s.boundaries[i] = Unknown          // i32 score, wrapped as the reference sums it
+ *   the wsconst_types post-filters on s                                              // they set NotWordBoundary, Unknown or not
+ *   for every i with given[i] != Unknown: s.boundaries[i] = given[i]                 // the caller's markers win, last
+ *   with predict_tags: fill_tags, then the PatternMatchTagger rules                  // tokens next to or across an Unknown get none
+ *   with keep_tags: every character that carries an input tag gets exactly its input tags   // replaces what the model or a rule put there
+ *   write_partial_annotation_text over the raw text; "\n"
+ *
+ * Definitions of this library, not of a reference command:
+ *   - markers: a given '|' / '-' is written as given, whatever the score or the post-filters say; a given ' ' is written
+ *     as '|' / '-' when the model is sure, as '-' when a post-filter cleared it, and stays ' ' otherwise;
+ *   - a character carries input tags when at least one of its tag fields is non-empty ("火/" and "火//" carry none, so
+ *     the model's and the rules' tags may appear there);
+ *   - a character's input tags are written as the reference writer writes a parsed sentence's tags: '/' + tag for every
+ *     field up to the last non-empty one, unescaped (sentence.rs:907-944).  In bytes: the character's tag region, from
+ *     the '/' that follows it to the marker that ends it (or the line's end), with every escaping '\' dropped, up to and
+ *     including the last content byte.  As in vpt_annotate_lines, a tag that holds ' ', '-', '|', '/' or '\' does not
+ *     read back;
+ *   - input tags stay at their character even when it does not end a token, and even next to a ' ': the reference
+ *     writer writes tags per character;
+ *   - keep_tags == 0: the input tags are parsed, checked and dropped, as vpt_tokenize_partial_lines drops them (for a
+ *     corpus whose first-round tags are the old model's guesses rather than an annotator's corrections);
+ *   - an empty line gives an empty output line; a malformed line stops the call with exactly vpt_tokenize_partial_lines'
+ *     errors and line numbers (UTF-8 first), and output delivered before the error ends at a line end;
+ *   - `margin` must not be negative (VPT_INVALID_ARGUMENT); with margin 0 only the caller's ' ' positions change, and
+ *     they become '|' or '-'.
+ * The parse, input tag regions, scoring, margin, post-filters, markers, tags, rules and writer run on the device.  Flags
+ * are checked as in vpt_tokenize_partial_lines; `out`, `out_capacity`, *out_len and *n_lines as there (the output of a
+ * line is at most that of its raw text in vpt_tokenize_lines_tags plus its input bytes).
+ * Not offered: a device-resident variant, score dumps, escaped tags, a scoring pass that skips given boundaries. */
+int vpt_reannotate_lines(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */, const uint8_t* utf8,
+                         size_t n_bytes, int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin,
+                         int keep_tags, uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines);
+
+/* A line stream of vpt_reannotate_lines: the same output, errors and line count on input fed in pieces, with the
+ * progress, memory and error rules of vpt_line_stream_new_partial. */
+int vpt_line_stream_new_reannotate(const vpt_predictor* predictor, const vpt_tag_rules* rules /* nullable */,
+                                   int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin, int keep_tags,
+                                   vpt_stream_write_fn write, void* ctx, vpt_line_stream** out);
 
 /* ---- Score dumps: the predict CLI's --scores and --tag-scores (predict/src/main.rs:66-93, 125-181) ------------------
  *

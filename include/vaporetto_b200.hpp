@@ -10,7 +10,7 @@
 //                                           iter_tokens, write_tokenized_text)
 //   vaporetto::CharacterBoundary / CharacterType   sentence.rs:9-29,70-82
 //   vaporetto::VaporettoError   errors.rs:15-38 (thrown as a C++ exception; `Result<_, VaporettoError>`)
-//   vaporetto::LineStream   (this library's own) tokenize_lines / evaluate_lines / tokenize_partial_lines / annotate_lines on input fed
+//   vaporetto::LineStream   (this library's own) tokenize_lines / evaluate_lines / tokenize_partial_lines / annotate_lines / reannotate_lines on input fed
 //                           in pieces, output to a sink
 // Where the reference panics (fill_tags on a predictor created with predict_tags = false, predictor.rs:547-551)
 // this mirror throws VaporettoError(InvalidArgument).
@@ -187,6 +187,28 @@ public:
             const int rc = vpt_annotate_lines(h_, detail::rules_handle(tag_rules), reinterpret_cast<const uint8_t*>(text.data()),
                                               text.size(), no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0, margin,
                                               reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl);
+            if (rc != 0 && attempt == 0 && n_out > out.size()) { out.assign(size_t(n_out) + 1, '\0'); continue; }  // long tag strings
+            detail::check(rc);
+            break;
+        }
+        out.resize(size_t(n_out));
+        return out;
+    }
+
+    /// Partially annotated lines in, partially annotated lines out (`vpt_reannotate_lines`): the caller's '|' / '-' and,
+    /// with `keep_tags`, the characters' input tags stay as written; the model decides the ' ' positions and leaves open
+    /// those whose score lies strictly between -margin and margin.  A malformed line throws, naming it.
+    std::string reannotate_lines(const std::string& text, int32_t margin = 0, bool keep_tags = true, bool no_norm = false,
+                                 uint32_t wsconst_types = 0, bool predict_tags = false,
+                                 const TagRules* tag_rules = nullptr) const {
+        size_t n_lines = 0;
+        for (char c : text) n_lines += c == '\n';
+        std::string out((predict_tags ? 19 : 3) * text.size() + n_lines + 1, '\0');
+        uint64_t n_out = 0, nl = 0;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            const int rc = vpt_reannotate_lines(h_, detail::rules_handle(tag_rules), reinterpret_cast<const uint8_t*>(text.data()),
+                                                text.size(), no_norm ? 1 : 0, wsconst_types, predict_tags ? 1 : 0, margin,
+                                                keep_tags ? 1 : 0, reinterpret_cast<uint8_t*>(&out[0]), out.size(), &n_out, &nl);
             if (rc != 0 && attempt == 0 && n_out > out.size()) { out.assign(size_t(n_out) + 1, '\0'); continue; }  // long tag strings
             detail::check(rc);
             break;
@@ -583,6 +605,18 @@ public:
         detail::check(vpt_line_stream_new_annotate(predictor.handle(), detail::rules_handle(tag_rules), no_norm ? 1 : 0,
                                                    wsconst_types, predict_tags ? 1 : 0, a.margin,
                                                    sink_ ? &LineStream::write : nullptr, this, &h_));
+    }
+    /// The stream of Predictor::reannotate_lines (`vpt_line_stream_new_reannotate`).
+    struct ReannotateLines {
+        int32_t margin = 0;
+        bool keep_tags = true;
+    };
+    LineStream(const Predictor& predictor, ReannotateLines a, Sink sink, bool no_norm = false, uint32_t wsconst_types = 0,
+               bool predict_tags = false, const TagRules* tag_rules = nullptr)
+        : sink_(std::move(sink)) {
+        detail::check(vpt_line_stream_new_reannotate(predictor.handle(), detail::rules_handle(tag_rules), no_norm ? 1 : 0,
+                                                     wsconst_types, predict_tags ? 1 : 0, a.margin, a.keep_tags ? 1 : 0,
+                                                     sink_ ? &LineStream::write : nullptr, this, &h_));
     }
     /// kind: VPT_STREAM_TOKENIZE (`sink` receives the tokenised lines) or VPT_STREAM_EVALUATE (`sink` may be empty).
     /// tag_rules: as in Predictor::tokenize_lines.  dumps: VPT_DUMP_SCORES | VPT_DUMP_TAG_SCORES, the predict CLI's

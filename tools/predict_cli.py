@@ -36,8 +36,13 @@ command with its 0-based line number (vpt_line_stream_new_partial).  It cannot b
 --write-partial-annotation is an extension too: the output lines are in the format of the reference's
 Sentence::write_partial_annotation_text ('|' a boundary, '-' none, ' ' unknown, tags unescaped), and --margin N leaves
 every boundary whose score lies strictly between -N and N unknown for an annotator to resolve (default 0: none); tokens
-next to an unknown boundary get no tags (vpt_line_stream_new_annotate).  It cannot be combined with --scores,
---tag-scores or --partial-annotation."""
+next to an unknown boundary get no tags (vpt_line_stream_new_annotate).  It cannot be combined with --scores or
+--tag-scores.
+
+--partial-annotation --write-partial-annotation re-annotates a partially annotated corpus, the second round of the
+domain-adaptation loop: the given '|' / '-' and every character's input tags are written back as given, the model
+decides each ' ' and leaves open those scoring strictly between -N and N (--margin N); --drop-input-tags drops the
+input tags instead, so that --predict-tags may fill them again (vpt_line_stream_new_reannotate)."""
 import argparse
 import os
 import select
@@ -118,6 +123,9 @@ def main(argv=None) -> int:
                          "the given markers are kept, the model decides the rest")
     ap.add_argument("--write-partial-annotation", action="store_true",
                     help="Extension: write partially annotated lines ('|' boundary, '-' none, ' ' unknown)")
+    ap.add_argument("--drop-input-tags", action="store_true",
+                    help="With --partial-annotation --write-partial-annotation: drop the input's tags instead of "
+                         "writing them back")
     ap.add_argument("--margin", type=int, default=0, metavar="N",
                     help="With --write-partial-annotation: boundaries scoring strictly between -N and N stay unknown")
     ap.add_argument("--device", type=int, default=0, help="CUDA device ordinal")
@@ -128,8 +136,10 @@ def main(argv=None) -> int:
         ap.error("--tag-scores needs --predict-tags")
     if args.partial_annotation and (args.scores or args.tag_scores):
         ap.error("--partial-annotation cannot be combined with --scores or --tag-scores")
-    if args.write_partial_annotation and (args.scores or args.tag_scores or args.partial_annotation):
-        ap.error("--write-partial-annotation cannot be combined with --scores, --tag-scores or --partial-annotation")
+    if args.write_partial_annotation and (args.scores or args.tag_scores):
+        ap.error("--write-partial-annotation cannot be combined with --scores or --tag-scores")
+    if args.drop_input_tags and not (args.partial_annotation and args.write_partial_annotation):
+        ap.error("--drop-input-tags needs --partial-annotation and --write-partial-annotation")
     if args.margin and not args.write_partial_annotation:
         ap.error("--margin needs --write-partial-annotation")
     if not 0 <= args.margin <= 2**31 - 1:
@@ -148,10 +158,11 @@ def main(argv=None) -> int:
     print("Start tokenization", file=sys.stderr)
     inp, out = sys.stdin.buffer, sys.stdout.buffer
     t0 = time.perf_counter()
-    kind = "partial" if args.partial_annotation else "annotate" if args.write_partial_annotation else "tokenize"
+    kind = ("reannotate" if args.partial_annotation and args.write_partial_annotation else
+            "partial" if args.partial_annotation else "annotate" if args.write_partial_annotation else "tokenize")
     with predictor.line_stream(kind=kind, no_norm=args.no_norm, wsconst="".join(args.wsconst), predict_tags=args.predict_tags,
                                tag_rules=tagger, scores=args.scores, tag_scores=args.tag_scores,
-                               margin=args.margin) as stream:
+                               margin=args.margin, keep_tags=not args.drop_input_tags) as stream:
         while True:
             data = inp.read1(READ_BYTES)
             if not data:

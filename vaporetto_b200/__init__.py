@@ -139,6 +139,10 @@ ABI = [
     ("vpt_annotate_lines", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, C.c_int32, _P, C.c_size_t,
                                      C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("vpt_line_stream_new_annotate", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, C.c_int32, _P, _P, C.POINTER(_P)]),
+    ("vpt_reannotate_lines", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, C.c_int, C.c_int32, C.c_int, _P,
+                                       C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("vpt_line_stream_new_reannotate", C.c_int, [_P, _P, C.c_int, C.c_uint32, C.c_int, C.c_int32, C.c_int, _P, _P,
+                                                 C.POINTER(_P)]),
     ("vpt_write_partial_annotation_text", C.c_int, [_P, _P, C.c_size_t, _P, _P, _P, _P, C.c_size_t, C.POINTER(C.c_uint64)]),
     ("vpt_token_spans", C.c_int, [_P, _P, _P, C.c_size_t, C.c_int, C.c_uint32, _P, _P, _P, _P, _P, C.c_size_t,
                                   C.POINTER(C.c_uint64)]),
@@ -600,6 +604,34 @@ class Predictor:
         _check(rc)
         return out[: n.value].tobytes(), int(nl.value)
 
+    def reannotate_lines(self, data, margin: int = 0, keep_tags: bool = True, no_norm: bool = False, wsconst: str = "",
+                         predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
+                         out: Optional[np.ndarray] = None):
+        """Partially annotated lines in, partially annotated lines out (vpt_reannotate_lines): every line is read as
+        tokenize_partial_lines reads it, and written as annotate_lines writes its lines.  The caller's '|' and '-' are
+        written as given; a ' ' becomes '|' or '-' where the model is sure (its score lies outside (-margin, margin), or
+        a `wsconst` post-filter decides it) and stays ' ' otherwise.  With `keep_tags`, every character whose tag fields
+        are not all empty gets exactly its input tags back (unescaped), in place of the model's and the rules' tags;
+        otherwise the input tags are dropped.  An empty line gives an empty output line; a malformed line raises
+        tokenize_partial_lines' VaporettoError.  Returns (bytes of the output lines, number of lines)."""
+        mask = _wsconst_mask(wsconst)
+        t = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else np.ascontiguousarray(data, np.uint8)
+        if out is None:
+            out = np.empty((2 + (16 if predict_tags else 0)) * t.size + int(np.count_nonzero(t == 10)) + 16, np.uint8)
+        n = C.c_uint64()
+        nl = C.c_uint64()
+        rules = tag_rules._handle() if tag_rules is not None else None
+        for _ in range(2):
+            rc = lib().vpt_reannotate_lines(self._h, rules, t.ctypes.data, t.size, int(no_norm), mask, int(predict_tags),
+                                            int(margin), int(keep_tags), out.ctypes.data, out.size, C.byref(n),
+                                            C.byref(nl))
+            if rc == 2 and n.value > out.size:
+                out = np.empty(n.value + 16, np.uint8)   # long tag strings: the call reported the size it needs
+                continue
+            break
+        _check(rc)
+        return out[: n.value].tobytes(), int(nl.value)
+
     def evaluate_lines(self, data, no_norm: bool = False, wsconst: str = "", predict_tags: bool = False,
                        per_line: bool = False):
         """The reference's `evaluate` command (evaluate/src/main.rs:69-195, vpt_evaluate_lines) over a buffer holding a
@@ -742,14 +774,16 @@ class Predictor:
 
     def line_stream(self, kind: str = "tokenize", no_norm: bool = False, wsconst: str = "",
                     predict_tags: bool = False, tag_rules: Optional["PatternMatchTagger"] = None,
-                    scores: bool = False, tag_scores: bool = False, margin: int = 0) -> "LineStream":
+                    scores: bool = False, tag_scores: bool = False, margin: int = 0,
+                    keep_tags: bool = True) -> "LineStream":
         """tokenize_lines (kind="tokenize"), evaluate_lines (kind="evaluate"), tokenize_partial_lines
-        (kind="partial") or annotate_lines (kind="annotate", with `margin`) on input fed in pieces of any size,
+        (kind="partial"), annotate_lines (kind="annotate", with `margin`) or reannotate_lines (kind="reannotate",
+        with `margin` and `keep_tags`) on input fed in pieces of any size,
         with host memory bounded by the pipeline, not by the input (vpt_line_stream_*): see LineStream.  `tag_rules`
         as in tokenize_lines.  `scores` / `tag_scores` (tokenize only; `tag_scores` needs predict_tags and a model with
         tag slots) add the predict CLI's --scores / --tag-scores dumps behind every token line
         (vpt_line_stream_new_scores)."""
-        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules, scores, tag_scores, margin)
+        return LineStream(self, kind, no_norm, wsconst, predict_tags, tag_rules, scores, tag_scores, margin, keep_tags)
 
 
 class LineStream:
@@ -762,9 +796,10 @@ class LineStream:
 
     def __init__(self, predictor: "Predictor", kind: str, no_norm: bool, wsconst: str, predict_tags: bool,
                  tag_rules: Optional["PatternMatchTagger"] = None, scores: bool = False, tag_scores: bool = False,
-                 margin: int = 0):
-        if kind not in STREAM_KINDS and kind not in ("partial", "annotate"):
-            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize', 'evaluate', 'partial' or 'annotate'")
+                 margin: int = 0, keep_tags: bool = True):
+        if kind not in STREAM_KINDS and kind not in ("partial", "annotate", "reannotate"):
+            raise VaporettoError(2, "InvalidArgumentError: kind: 'tokenize', 'evaluate', 'partial', 'annotate' or "
+                                    "'reannotate'")
         dumps = (DUMP_SCORES if scores else 0) | (DUMP_TAG_SCORES if tag_scores else 0)
         if dumps and kind != "tokenize":
             raise VaporettoError(2, "InvalidArgumentError: scores, tag_scores: kind='tokenize' only")
@@ -783,6 +818,10 @@ class LineStream:
         elif kind == "annotate":
             _check(lib().vpt_line_stream_new_annotate(predictor._h, rules, int(no_norm), mask, int(predict_tags),
                                                       int(margin), C.cast(self._write, _P), None, C.byref(h)))
+        elif kind == "reannotate":
+            _check(lib().vpt_line_stream_new_reannotate(predictor._h, rules, int(no_norm), mask, int(predict_tags),
+                                                        int(margin), int(keep_tags), C.cast(self._write, _P), None,
+                                                        C.byref(h)))
         elif dumps:
             _check(lib().vpt_line_stream_new_scores(predictor._h, rules, int(no_norm), mask, int(predict_tags), dumps,
                                                     C.cast(self._write, _P), None, C.byref(h)))

@@ -13,7 +13,10 @@
 //     (separate kernels, so that those keep their compiled code): one warp per sentence, 128 bytes per step, one CTA per 64-sentence group with a decoupled look-back for
 //     the group's output offset.  A marker goes before every character after the first; a token's "/tag" suffix goes
 //     in front of the marker after its last character (the last token's in front of the '\n').  Nothing is escaped:
-//     the tag strings, stored escaped (tags_build.cpp, tag_rules.hpp), are copied without their '\' escapes.
+//     the tag strings, stored escaped (tags_build.cpp, tag_rules.hpp), are copied without their '\' escapes;
+//   * k_pa_rewrite<kTags, kRules> (vpt_reannotate_lines): k_pa_write's body with the caller's input tags, which go after
+//     any character that carries them (k_part_tags, partial.cu, found where in the chunk's input), in place of the
+//     suffix of the token it ends.
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -87,6 +90,13 @@ __global__ void __launch_bounds__(kAnThreads) k_pa_untag(AnnArgs a) {
     }
 }
 
+// vpt_reannotate_lines: the chunk's input and the input tag region of every character (k_part_tags)
+struct InTags {
+    const uint8_t* input = nullptr;
+    const uint2* regions = nullptr;
+    const uint64_t* char_offsets = nullptr;
+};
+
 // The bytes of a stored (escaped) tag string without its escapes
 __device__ __forceinline__ uint32_t unescaped_len(const uint8_t* __restrict__ src, uint2 ref) {
     uint32_t n = 0;
@@ -135,18 +145,22 @@ __device__ __forceinline__ uint32_t pa_suffix(const TokArgs& t, const TagRuleArg
 // character k of the sentence goes to x + k + (suffix bytes of the tokens that ended before character k); the marker of
 // character k >= 1 goes right before its first byte, and the suffix of the token that ends at character k - 1 right
 // before that marker.
-template <bool kWrite, bool kTags, bool kRules>
+// kIn (vpt_reannotate_lines): a character whose input tag region (`in`) is not empty gets it, unescaped, right after
+// it, in place of the suffix of the token it ends; the suffix bytes in front of character k are then those of character
+// k - 1, of either kind.
+template <bool kWrite, bool kTags, bool kRules, bool kIn = false>
 __device__ __forceinline__ uint32_t pa_sentence(const TokArgs& t, const TagRuleArgs& ra, const uint8_t* __restrict__ marks,
                                                 uint64_t s, uint64_t o0, uint64_t o1, uint32_t trim, uint32_t nch,
-                                                uint8_t* __restrict__ out, int lane) {
+                                                uint8_t* __restrict__ out, int lane, const InTags& in = InTags()) {
     const uint64_t a0 = o0 & ~3ull;
     const uint32_t b0 = uint32_t(o0 - a0), b1 = uint32_t(o1 - a0) - trim;
-    if (!kWrite && !kTags) return (b1 - b0) + nch - 1;
+    if (!kWrite && !kTags && !kIn) return (b1 - b0) + nch - 1;
     const uint8_t* __restrict__ base = t.text + a0;
     const uint64_t bo = t.bound_offsets[s];
     const uint8_t* __restrict__ bnd = t.boundaries + bo;
     const uint8_t* __restrict__ mk = marks + bo;
     const uint64_t rec0 = kTags ? t.tok_base[s] : 0;
+    const uint2* __restrict__ reg = kIn ? in.regions + in.char_offsets[s] : nullptr;
     uint32_t chars = 0, extra = 0, toks = 0;  // characters / suffix bytes / tokens ended, before this window
     for (uint32_t w0 = 0; w0 < b1; w0 += 128) {
         const uint32_t addr = w0 + 4u * uint32_t(lane);
@@ -173,18 +187,37 @@ __device__ __forceinline__ uint32_t pa_sentence(const TokArgs& t, const TagRuleA
         const uint32_t nwb = __popc(wb80);
         const uint32_t wb_incl = kTags ? warp_incl_scan_u32(nwb, lane) : 0u;
         uint32_t sl[4] = {0, 0, 0, 0}, sl_sum = 0;
+        uint32_t in80s = 0;  // kIn: the character starts whose previous character has input tags
+        uint2 rg[4];
+        if (kIn) {
+            uint32_t k = chars + st_incl - nst;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (st80 & (0x80u << (8 * j))) {
+                    rg[j] = k >= 1 ? reg[k - 1] : make_uint2(0, 0);
+                    if (rg[j].y) {
+                        in80s |= 0x80u << (8 * j);
+                        sl[j] = unescaped_len(in.input, rg[j]);
+                        sl_sum += sl[j];
+                    }
+                    ++k;
+                }
+            }
+        }
         if (kTags) {
             uint64_t rec = rec0 + toks + wb_incl - nwb;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 if (wb80 & (0x80u << (8 * j))) {
-                    sl[j] = pa_suffix<false, kRules>(t, ra, rec, nullptr);
-                    sl_sum += sl[j];
+                    if (!(kIn && (in80s & (0x80u << (8 * j))))) {
+                        sl[j] = pa_suffix<false, kRules>(t, ra, rec, nullptr);
+                        sl_sum += sl[j];
+                    }
                     ++rec;
                 }
             }
         }
-        const uint32_t sl_incl = kTags ? warp_incl_scan_u32(sl_sum, lane) : 0u;
+        const uint32_t sl_incl = (kTags || kIn) ? warp_incl_scan_u32(sl_sum, lane) : 0u;
         if (kWrite) {
             uint32_t k = chars + st_incl - nst;        // the next character that starts in this word
             uint32_t e = extra + sl_incl - sl_sum;     // suffix bytes in front of character k - 1
@@ -196,7 +229,11 @@ __device__ __forceinline__ uint32_t pa_sentence(const TokArgs& t, const TagRuleA
                 const uint32_t x = addr + uint32_t(j) - b0;
                 if (st80 & bit) {
                     if (k >= 1) {
-                        if (kTags && (wb80 & bit)) {
+                        if (kIn && (in80s & bit)) {
+                            e += sl[j];
+                            unescaped_copy(in.input, rg[j], out + x + k + e - 1 - sl[j]);
+                            if (kTags && (wb80 & bit)) ++rec;
+                        } else if (kTags && (wb80 & bit)) {
                             e += sl[j];
                             pa_suffix<true, kRules>(t, ra, rec, out + x + k + e - 1 - sl[j]);
                             ++rec;
@@ -209,13 +246,16 @@ __device__ __forceinline__ uint32_t pa_sentence(const TokArgs& t, const TagRuleA
             }
         }
         chars += __shfl_sync(kFull, st_incl, 31);
-        if (kTags) {
-            extra += __shfl_sync(kFull, sl_incl, 31);
-            toks += __shfl_sync(kFull, wb_incl, 31);
-        }
+        if (kTags || kIn) extra += __shfl_sync(kFull, sl_incl, 31);
+        if (kTags) toks += __shfl_sync(kFull, wb_incl, 31);
     }
     uint32_t len = (b1 - b0) + nch - 1 + extra;
-    if (kTags && nch > 0) {
+    const uint2 last_in = kIn && nch > 0 ? reg[nch - 1] : make_uint2(0, 0);
+    if (kIn && last_in.y) {
+        const uint32_t last = unescaped_len(in.input, last_in);
+        if (kWrite && lane == 0) unescaped_copy(in.input, last_in, out + len);
+        len += last;
+    } else if (kTags && nch > 0) {
         const uint32_t last = pa_suffix<false, kRules>(t, ra, rec0 + toks, nullptr);
         if (kWrite && lane == 0) pa_suffix<true, kRules>(t, ra, rec0 + toks, out + len);
         len += last;
@@ -223,8 +263,9 @@ __device__ __forceinline__ uint32_t pa_sentence(const TokArgs& t, const TagRuleA
     return len;
 }
 
-template <bool kTags, bool kRules>
-__global__ void __launch_bounds__(kAnThreads, 1) k_pa_write(TokArgs t, uint64_t ngroups, TagRuleArgs ra, const uint8_t* __restrict__ marks) {
+template <bool kTags, bool kRules, bool kIn>
+__device__ __forceinline__ void pa_write(const TokArgs& t, uint64_t ngroups, const TagRuleArgs& ra,
+                                         const uint8_t* __restrict__ marks, const InTags& in) {
     __shared__ uint64_t s_off[kGroup + 1];
     __shared__ uint32_t s_nch[kGroup];
     __shared__ uint32_t s_len[kGroup], s_excl[kGroup];
@@ -250,8 +291,8 @@ __global__ void __launch_bounds__(kAnThreads, 1) k_pa_write(TokArgs t, uint64_t 
     for (int i = warp; i < ns; i += kWarps) {
         uint32_t len = 1;  // the '\n'
         if (!s_bad[i])
-            len += pa_sentence<false, kTags, kRules>(t, ra, marks, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i],
-                                                     nullptr, lane);
+            len += pa_sentence<false, kTags, kRules, kIn>(t, ra, marks, gbase + i, s_off[i], s_off[i + 1], s_trim[i],
+                                                          s_nch[i], nullptr, lane, in);
         if (lane == 0) s_len[i] = len;
     }
     __syncthreads();
@@ -299,9 +340,21 @@ __global__ void __launch_bounds__(kAnThreads, 1) k_pa_write(TokArgs t, uint64_t 
         uint8_t* __restrict__ out = t.out + gout + s_excl[i];
         if (lane == 0) out[s_len[i] - 1] = 0x0A;
         if (!s_bad[i])
-            pa_sentence<true, kTags, kRules>(t, ra, marks, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i], out,
-                                             lane);
+            pa_sentence<true, kTags, kRules, kIn>(t, ra, marks, gbase + i, s_off[i], s_off[i + 1], s_trim[i], s_nch[i],
+                                                  out, lane, in);
     }
+}
+
+template <bool kTags, bool kRules>
+__global__ void __launch_bounds__(kAnThreads, 1) k_pa_write(TokArgs t, uint64_t ngroups, TagRuleArgs ra, const uint8_t* __restrict__ marks) {
+    pa_write<kTags, kRules, false>(t, ngroups, ra, marks, InTags());
+}
+
+// k_pa_write with the input tags of vpt_reannotate_lines
+template <bool kTags, bool kRules>
+__global__ void __launch_bounds__(kAnThreads, 1) k_pa_rewrite(TokArgs t, uint64_t ngroups, TagRuleArgs ra,
+                                                              const uint8_t* __restrict__ marks, InTags in) {
+    pa_write<kTags, kRules, true>(t, ngroups, ra, marks, in);
 }
 
 unsigned warp_blocks(uint64_t n) { return unsigned((n + kWarps - 1) / kWarps); }
@@ -335,6 +388,22 @@ cudaError_t launch_pa_write(const TokArgs& t, const TagRuleArgs& ra, const uint8
     if (t.tok_base && ra.tok_rule) k_pa_write<true, true><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks);
     else if (t.tok_base) k_pa_write<true, false><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks);
     else k_pa_write<false, false><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pa_rewrite(const TokArgs& t, const TagRuleArgs& ra, const uint8_t* marks, const uint8_t* input,
+                              const uint2* regions, const uint64_t* char_offsets, cudaStream_t stream) {
+    if (t.n_sent == 0) return cudaMemsetAsync(t.total, 0, 8, stream);
+    const uint64_t ngroups = (t.n_sent + kGroup - 1) / kGroup;
+    cudaError_t e = cudaMemsetAsync(t.tok_state, 0, 8 * (ngroups + 1), stream);
+    if (e != cudaSuccess) return e;
+    InTags in;
+    in.input = input;
+    in.regions = regions;
+    in.char_offsets = char_offsets;
+    if (t.tok_base && ra.tok_rule) k_pa_rewrite<true, true><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks, in);
+    else if (t.tok_base) k_pa_rewrite<true, false><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks, in);
+    else k_pa_rewrite<false, false><<<unsigned(ngroups), kAnThreads, 0, stream>>>(t, ngroups, ra, marks, in);
     return cudaGetLastError();
 }
 

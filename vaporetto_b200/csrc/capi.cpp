@@ -85,7 +85,8 @@ struct Scratch {
     void* d_stage = nullptr; size_t stage_cap = 0;
     void* d_dsize = nullptr; size_t dsize_cap = 0;
     // gold corpus and metrics (vpt_evaluate_lines); the partial parse (vpt_tokenize_partial_lines) uses gtext, goff,
-    // gcoff, gbnd (its marker codes) and evtot (its error key); vpt_annotate_lines keeps its output markers in gbnd
+    // gcoff, gbnd (its marker codes) and evtot (its error key); vpt_annotate_lines keeps its output markers in gbnd,
+    // vpt_reannotate_lines in pmark (gbnd holds the input's), and its input tag regions in ptag
     void* d_gtext = nullptr; size_t gtext_cap = 0;
     void* d_goff = nullptr; size_t goff_cap = 0;
     void* d_gcoff = nullptr; size_t gcoff_cap = 0;
@@ -94,6 +95,8 @@ struct Scratch {
     void* d_gw = nullptr; size_t gw_cap = 0;
     void* d_lc = nullptr; size_t lc_cap = 0;
     void* d_evtot = nullptr; size_t evtot_cap = 0;
+    void* d_pmark = nullptr; size_t pmark_cap = 0;
+    void* d_ptag = nullptr; size_t ptag_cap = 0;
     uint64_t* h_eval = nullptr;    // pinned, kEvalTotals + 1 x u64: a chunk's totals and error key
     uint64_t* h_totals = nullptr;  // pinned, 10 x u64: boundaries, chars, lines, output bytes, tokens (score dumps: the
                                    // writer's token line bytes), first bit word, rule suffix bytes, tag scores, then the
@@ -105,7 +108,7 @@ struct Scratch {
         for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
                         d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends, d_trule,
                         d_scoff, d_scblk, d_tagsc, d_stage, d_dsize,
-                        d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot})
+                        d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot, d_pmark, d_ptag})
             if (p) cudaFree(p);
         if (h_totals) cudaFreeHost(h_totals);
         if (h_eval) cudaFreeHost(h_eval);
@@ -1131,16 +1134,18 @@ struct LineChunk {
 // What a line loop computes: the flags of vpt_tokenize_lines*, vpt_evaluate_lines or vpt_line_stream_new, checked
 constexpr int kJobPartial = 2;  // vpt_tokenize_partial_lines / vpt_line_stream_new_partial (no public stream kind)
 constexpr int kJobAnnotate = 3;  // vpt_annotate_lines / vpt_line_stream_new_annotate (no public stream kind)
+constexpr int kJobReannotate = 4;  // vpt_reannotate_lines / vpt_line_stream_new_reannotate (no public stream kind)
 
 struct LineJob {
-    int kind;          // VPT_STREAM_TOKENIZE, VPT_STREAM_EVALUATE, kJobPartial or kJobAnnotate
+    int kind;          // VPT_STREAM_TOKENIZE, VPT_STREAM_EVALUATE, kJobPartial, kJobAnnotate or kJobReannotate
     bool normalize;    // KyteaFullwidthFilter (no_norm == 0)
     uint32_t wsconst;  // post-filters (VPT_WSCONST_*)
     bool tags;         // tags predicted on the device
     int tag_mode;      // evaluate: how the system's tags compare with the gold's (kTags*)
     const vpt_tag_rules* rules = nullptr;  // PatternMatchTagger after fill_tags (tokenize with tags and rules only)
     uint32_t dumps = 0;    // tokenize: the predict CLI's --scores / --tag-scores (kDumpScores | kDumpTagScores, dump.hpp)
-    int32_t margin = 0;    // annotate: boundaries with -margin < score < margin are left Unknown
+    int32_t margin = 0;    // (re)annotate: boundaries with -margin < score < margin are left Unknown
+    bool keep_tags = false;  // reannotate: characters with input tags get them back
 };
 
 // stage 0 of a chunk: H2D of its `nbytes` at `bytes`, newline counts, the number of lines to pinned host memory
@@ -1599,7 +1604,9 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
 
 // stage 1 of a chunk of partially annotated lines: line offsets, the parse (raw text, markers, error key), count +
 // score + post-filters on the raw text, the caller's markers, tags, the tokenized writer over the raw text; the output
-// size and the error key to pinned host memory
+// size and the error key to pinned host memory.  kJobReannotate: the margin and the output markers as lines_stage1's
+// annotate job, with the caller's markers applied after the post-filters, and the partial-annotation writer; with
+// keep_tags the input tag region of every character (k_part_tags) goes to that writer.
 void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
     cudaStream_t st = s.stream;
     const size_t n = split_lines(s, ch);
@@ -1614,8 +1621,13 @@ void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
     Scratch::ensure(s.d_gbnd, s.gbnd_cap, nb + 4);
     Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
-    // as lines_stage1: the raw bytes bound the output of the writer (with tags, the longest suffix per token)
+    // as lines_stage1: the raw bytes bound the output of the writer (with tags, the longest suffix per token).  The
+    // reannotate writer's line is its raw text, a marker per character after the first, the written input tags and the
+    // model's suffixes.  The written input tags of a character are at most the bytes of its tag region, and the raw text,
+    // the markers and the tag regions are disjoint parts of the input line: all three together take at most the line's
+    // input bytes, so the same bound holds.
     const size_t out_need = 3 * nb + n + 4 + (job.tags ? nb * p.dt.max_suffix : 0);
+    const bool reannotate = job.kind == kJobReannotate;
     Scratch::ensure(s.d_out, s.out_cap, out_need);
     PartArgs e;
     e.text = ch.sp.text;
@@ -1631,12 +1643,30 @@ void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     e.err = static_cast<uint64_t*>(s.d_evtot) + kEvalTotals;
     cuda_check(cudaMemsetAsync(e.err, 0xFF, 8, st), "cudaMemset");
     cuda_check(launch_part_parse(e, st), "launch(part parse)");
+    PartTagArgs pt;
+    if (reannotate && job.keep_tags) {
+        // every character of a line is followed by a marker or ends the line: at most (nb + 1) / 2 characters
+        Scratch::ensure(s.d_ptag, s.ptag_cap, 8 * ((nb + 1) / 2 + 2));
+        pt.text = e.text;
+        pt.offsets = e.offsets;
+        pt.trims = e.trims;
+        pt.n_sent = n;
+        pt.char_offsets = e.char_offsets;
+        pt.regions = static_cast<uint2*>(s.d_ptag);
+        cuda_check(launch_part_tags(pt, st), "launch(part tags)");
+    }
+    AnnArgs ann;
+    if (reannotate) {
+        Scratch::ensure(s.d_pmark, s.pmark_cap, nb + 4);
+        ann.margin = job.margin;
+        ann.marks = static_cast<uint8_t*>(s.d_pmark);
+    }
     BatchArgs a;
     a.text = e.surface;
     a.offsets = e.surf_offsets;
     a.n_sent = n;
     TagRuleArgs ra;
-    TokArgs t = predict_lines(p, s, ch, a, nb, job, &ra, nullptr, &e);
+    TokArgs t = predict_lines(p, s, ch, a, nb, job, &ra, nullptr, &e, reannotate ? &ann : nullptr);
     if (ra.tok_rule) {
         // as lines_stage1: the rules' share of the output is sized from the suffixes the chunk's tokens matched
         cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
@@ -1651,7 +1681,9 @@ void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     t.total = t.tok_state + ng + 1;
     t.total_host = &s.h_totals[3];
     t.out = static_cast<uint8_t*>(s.d_out);
-    cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
+    if (pt.regions) cuda_check(launch_pa_rewrite(t, ra, ann.marks, e.text, pt.regions, e.char_offsets, st), "launch(reannotate)");
+    else if (reannotate) cuda_check(launch_pa_write(t, ra, ann.marks, st), "launch(annotate)");
+    else cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
     cuda_check(cudaMemcpyAsync(&s.h_eval[kEvalTotals], e.err, 8, cudaMemcpyDeviceToHost, st), "D2H(error key)");
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
@@ -1766,7 +1798,7 @@ struct LineRing {
         Scratch& s = *sl.lease->s;
         if (job.kind == VPT_STREAM_TOKENIZE || job.kind == kJobAnnotate) {
             lines_stage1(p, s, sl.ch, job);
-        } else if (job.kind == kJobPartial) {
+        } else if (job.kind == kJobPartial || job.kind == kJobReannotate) {
             part_stage1(p, s, sl.ch, job);
         } else {
             uint32_t* counts = nullptr;
@@ -1803,7 +1835,7 @@ struct LineRing {
                                                   " (line " + std::to_string(line) + ")");
             }
             for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
-        } else if (job.kind == kJobPartial) {
+        } else if (job.kind == kJobPartial || job.kind == kJobReannotate) {
             const uint64_t key = s.h_eval[kEvalTotals];
             if (key != kGoldNoError) {
                 const uint64_t l = key >> 34;
@@ -1872,16 +1904,18 @@ struct LineRing {
 
 int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types, bool tags,
                         uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out,
-                        const vpt_tag_rules* rules = nullptr, int kind = VPT_STREAM_TOKENIZE, int32_t margin = 0) {
+                        const vpt_tag_rules* rules = nullptr, int kind = VPT_STREAM_TOKENIZE, int32_t margin = 0,
+                        bool keep_tags = false) {
     VPT_API_BEGIN
     LineJob job = line_job(p, kind, no_norm, wsconst_types, tags, rules);
     job.margin = margin;
+    job.keep_tags = keep_tags;
     if (out_len) *out_len = 0;
     if (n_lines_out) *n_lines_out = 0;
     if (n_bytes && !utf8) throw Error(kInvalidArgument, "InvalidArgumentError: utf8: must not be NULL");
     if (n_bytes == 0) return kOk;
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
-    LineRing ring(*p, job, kind == kJobPartial ? "partial" : kind == kJobAnnotate ? "annotate" : "lines");
+    LineRing ring(*p, job, kind == kJobPartial ? "partial" : kind == kJobAnnotate ? "annotate" : kind == kJobReannotate ? "reannotate" : "lines");
     uint64_t total = 0;  // counts on past an overflow: *out_len is the size needed
     bool overflow = false;
     ring.run(utf8, n_bytes, [&](LineRing::Slot& sl) {
@@ -1984,6 +2018,18 @@ int vpt_annotate_lines(const vpt_predictor* p, const vpt_tag_rules* rules, const
     }
     return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, predict_tags != 0, out, out_capacity, out_len,
                                n_lines_out, rules, kJobAnnotate, margin);
+}
+
+int vpt_reannotate_lines(const vpt_predictor* p, const vpt_tag_rules* rules, const uint8_t* utf8, size_t n_bytes,
+                         int no_norm, uint32_t wsconst_types, int predict_tags, int32_t margin, int keep_tags,
+                         uint8_t* out, size_t out_capacity, uint64_t* out_len, uint64_t* n_lines_out) {
+    if (margin < 0) {
+        if (out_len) *out_len = 0;
+        if (n_lines_out) *n_lines_out = 0;
+        return fail(Error(kInvalidArgument, "InvalidArgumentError: margin: must not be negative"));
+    }
+    return tokenize_lines_impl(p, utf8, n_bytes, no_norm, wsconst_types, predict_tags != 0, out, out_capacity, out_len,
+                               n_lines_out, rules, kJobReannotate, margin, keep_tags != 0);
 }
 
 int vpt_evaluate_lines(const vpt_predictor* p, const uint8_t* utf8, size_t n_bytes, int no_norm, uint32_t wsconst_types,
@@ -2219,6 +2265,23 @@ int vpt_line_stream_new_annotate(const vpt_predictor* p, const vpt_tag_rules* ru
     LineJob job = line_job(p, kJobAnnotate, no_norm, wsconst_types, predict_tags != 0, rules);
     if (margin < 0) throw Error(kInvalidArgument, "InvalidArgumentError: margin: must not be negative");
     job.margin = margin;
+    if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
+    cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
+    *out = new vpt_line_stream(p, job, write, ctx);
+    return kOk;
+    VPT_API_END
+}
+
+int vpt_line_stream_new_reannotate(const vpt_predictor* p, const vpt_tag_rules* rules, int no_norm,
+                                   uint32_t wsconst_types, int predict_tags, int32_t margin, int keep_tags,
+                                   vpt_stream_write_fn write, void* ctx, vpt_line_stream** out) {
+    VPT_API_BEGIN
+    if (!out) throw Error(kInvalidArgument, "InvalidArgumentError: out: must not be NULL");
+    *out = nullptr;
+    LineJob job = line_job(p, kJobReannotate, no_norm, wsconst_types, predict_tags != 0, rules);
+    if (margin < 0) throw Error(kInvalidArgument, "InvalidArgumentError: margin: must not be negative");
+    job.margin = margin;
+    job.keep_tags = keep_tags != 0;
     if (!write) throw Error(kInvalidArgument, "InvalidArgumentError: write: must not be NULL");
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     *out = new vpt_line_stream(p, job, write, ctx);

@@ -238,6 +238,19 @@ cudaError_t launch_part_parse(const PartArgs& e, cudaStream_t stream);
 // every given '|' / '-' over the boundary it marks
 cudaError_t launch_part_apply(const PartArgs& e, cudaStream_t stream);
 
+// k_part_tags: the input tags of every character (vpt_reannotate_lines), as the byte range of the chunk's input that
+// holds them (partial_parse.hpp, pa_tag_region)
+struct PartTagArgs {
+    const uint8_t* text = nullptr;          // the chunk's input, as PartArgs; kept on the device until the writer ran
+    const uint64_t* offsets = nullptr;      // [n_sent + 1]
+    const uint8_t* trims = nullptr;         // [n_sent]
+    uint64_t n_sent = 0;
+    const uint64_t* char_offsets = nullptr; // [n_sent + 1] from k_part_parse
+    uint2* regions = nullptr;               // [characters] out, at char_offsets[line] + k: {first byte in `text`, bytes
+                                            // up to and including the last content byte}; y == 0: no input tags
+};
+cudaError_t launch_part_tags(const PartTagArgs& e, cudaStream_t stream);
+
 // ---- annotate.cu: partially annotated output (Sentence::write_partial_annotation_text, vpt_annotate_lines) ------------
 struct AnnArgs {
     int32_t margin = 0;                     // boundaries with -margin < score < margin become Unknown (0: none)
@@ -264,6 +277,11 @@ struct TagRuleArgs;
 // launch_tokenize_rules in the partial-annotation format: the markers from `marks`, the tags of TokArgs (tok_base
 // non-null) and of the rules (ra.tok_rule non-null) unescaped; zeroes tok_state[0 .. n_groups] (ticket included)
 cudaError_t launch_pa_write(const TokArgs& t, const TagRuleArgs& ra, const uint8_t* marks, cudaStream_t stream);
+// launch_pa_write with the caller's input tags (vpt_reannotate_lines): every character whose region (PartTagArgs, at
+// regions[char_offsets[line] + k]) is not empty gets the bytes of `input` it names, unescaped, after it, in place of
+// the suffix of the token it ends
+cudaError_t launch_pa_rewrite(const TokArgs& t, const TagRuleArgs& ra, const uint8_t* marks, const uint8_t* input,
+                              const uint2* regions, const uint64_t* char_offsets, cudaStream_t stream);
 
 // ---- spans.cu: documents -> token byte spans (vaporetto_tantivy's token_stream, vpt_token_spans) --------------------
 struct SpanArgs {

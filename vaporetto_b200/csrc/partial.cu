@@ -209,7 +209,111 @@ __global__ void __launch_bounds__(kPaThreads) k_part_apply(PartArgs e) {
     }
 }
 
+// One warp per line, 128 bytes per step, as part_line: the automaton's state before every byte from the same scan, then
+// every byte's tag class (pa_tag_class).  Each lane walks its bytes from the max of the carried walk and the lanes before
+// it (pa_tag_max); at every marker after a character, and at the line's end, the character's region is written.  Lines
+// with an error (the call fails on them) still write only inside their characters.
+__global__ void __launch_bounds__(kPaThreads) k_part_tags(PartTagArgs e) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t l = uint64_t(blockIdx.x) * kWarps + warp;
+    if (l >= e.n_sent) return;
+    const uint64_t o0 = e.offsets[l], o1 = e.offsets[l + 1];
+    const uint64_t a0 = o0 & ~3ull;
+    const uint32_t b0 = uint32_t(o0 - a0), b1 = uint32_t(o1 - a0) - e.trims[l];
+    if (b1 <= b0) return;
+    const uint8_t* __restrict__ base = e.text + a0;
+    uint2* __restrict__ regions = e.regions + e.char_offsets[l];
+    uint32_t c_state = kPaChar, chars = 0;
+    PaTagRun carry;
+    for (uint32_t w0 = 0; w0 < b1; w0 += 128) {
+        const uint32_t addr = w0 + 4u * uint32_t(lane);
+        uint32_t lo = 0, in80 = 0;
+        if (addr < b1) {
+            lo = __ldg(reinterpret_cast<const uint32_t*>(base + addr));
+            in80 = inside80(addr, b0, b1);
+        }
+        const uint32_t m = pa_word_map(lo, in80);
+        uint32_t incl = m;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t o = __shfl_up_sync(kFull, incl, d);
+            if (lane >= d) incl = pa_compose(o, incl);
+        }
+        uint32_t x = __shfl_up_sync(kFull, incl, 1);
+        if (lane == 0) x = kPaIdentity;
+        const uint32_t s0 = pa_apply(x, c_state);
+        // the lane's own walk from nothing: its character starts and its maxima
+        uint32_t s = s0, st80 = 0;
+        PaTagRun own;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t bit = 0x80u << (8 * j);
+            if (!(in80 & bit)) continue;
+            const uint32_t b = (lo >> (8 * j)) & 0xFFu;
+            const PaByte pb = pa_byte(s, b);
+            if (pb.start) st80 |= bit;
+            pa_tag_step(own, pb.start, pa_tag_class(s, b), addr + uint32_t(j) - b0);
+            s = pb.next;
+        }
+        const uint32_t nst = __popc(st80);
+        const uint32_t st_incl = warp_incl_scan_u32(nst, lane);
+        // the walk before the lane: max over the carry and the lanes before it
+        PaTagRun run = own;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            PaTagRun o;
+            o.start = __shfl_up_sync(kFull, run.start, d);
+            o.open = __shfl_up_sync(kFull, run.open, d);
+            o.content = __shfl_up_sync(kFull, run.content, d);
+            if (lane >= d) pa_tag_max(run, o);
+        }
+        PaTagRun before;
+        before.start = __shfl_up_sync(kFull, run.start, 1);
+        before.open = __shfl_up_sync(kFull, run.open, 1);
+        before.content = __shfl_up_sync(kFull, run.content, 1);
+        if (lane == 0) before = PaTagRun();
+        pa_tag_max(before, carry);
+        // the walk again, writing the region of the character before every marker
+        uint32_t k = chars + st_incl - nst;  // characters of the line before this byte
+        s = s0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t bit = 0x80u << (8 * j);
+            if (!(in80 & bit)) continue;
+            const uint32_t b = (lo >> (8 * j)) & 0xFFu;
+            const uint32_t cls = pa_tag_class(s, b);
+            if (st80 & bit) ++k;
+            pa_tag_step(before, (st80 & bit) != 0, cls, addr + uint32_t(j) - b0);
+            if (cls == kPaTagClose) {
+                uint32_t first;
+                const uint32_t len = pa_tag_region(before, first);
+                regions[k - 1] = make_uint2(uint32_t(a0) + b0 + first, len);
+            }
+            s = pa_apply(pa_byte_map(b), s);
+        }
+        c_state = pa_apply(__shfl_sync(kFull, incl, 31), c_state);
+        chars += __shfl_sync(kFull, st_incl, 31);
+        PaTagRun step;
+        step.start = __shfl_sync(kFull, run.start, 31);
+        step.open = __shfl_sync(kFull, run.open, 31);
+        step.content = __shfl_sync(kFull, run.content, 31);
+        pa_tag_max(carry, step);
+    }
+    // the last character: its region ends with the line
+    if (lane == 0 && chars > 0 && c_state != kPaChar && c_state != kPaErr) {
+        uint32_t first;
+        const uint32_t len = pa_tag_region(carry, first);
+        regions[chars - 1] = make_uint2(uint32_t(a0) + b0 + first, len);
+    }
+}
+
 }  // namespace
+
+cudaError_t launch_part_tags(const PartTagArgs& e, cudaStream_t stream) {
+    if (e.n_sent == 0) return cudaSuccess;
+    k_part_tags<<<unsigned((e.n_sent + kWarps - 1) / kWarps), kPaThreads, 0, stream>>>(e);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_part_parse(const PartArgs& e, cudaStream_t stream) {
     if (e.n_sent == 0) return cudaSuccess;

@@ -87,4 +87,53 @@ VPT_HD PaByte pa_byte(uint32_t s, uint32_t b) {
     return r;
 }
 
+// ---- input tags (k_part_tags, vpt_reannotate_lines) ----------------------------------------------------------------
+//
+// A character's input tags are written back as the reference writes a parsed sentence's tags (sentence.rs:907-944):
+// '/' + tag for every field up to the last non-empty one, unescaped.  In bytes that is its tag region -- from the '/'
+// that opens it to the marker that ends it, or to the line's end -- with every escaping '\' dropped, up to and including
+// the last content byte.  What a byte is to that region, read in state `s` (a continuation byte is read in the state
+// its lead byte left, so it follows its lead byte):
+enum PaTagClass : uint32_t {
+    kPaTagNone = 0,     // not part of a tag region
+    kPaTagOpen = 1,     // the '/' that opens the region (read in kPaMark): written
+    kPaTagSep = 2,      // a later '/' separator: written
+    kPaTagDrop = 3,     // an escaping '\': dropped
+    kPaTagContent = 4,  // tag content, escaped or not: written
+    kPaTagClose = 5,    // the marker after the character (with or without a region)
+};
+
+VPT_HD uint32_t pa_tag_class(uint32_t s, uint32_t b) {
+    if (s == kPaTagEsc) return kPaTagContent;
+    if (s == kPaMark) return b == 0x2Fu ? kPaTagOpen : pa_marker(b) ? kPaTagClose : kPaTagNone;
+    if (s != kPaTag) return kPaTagNone;
+    return b == 0x2Fu ? kPaTagSep : b == 0x5Cu ? kPaTagDrop : pa_marker(b) ? kPaTagClose : kPaTagContent;
+}
+
+// Where the walk over a line is: the last character start, region open and content byte before it (position + 1 in
+// the line; 0: none).  Positions only grow, so the walk over bytes [a, c) is the elementwise max of its walks over
+// [a, b) and [b, c): lanes and steps combine by max.
+struct PaTagRun {
+    uint32_t start = 0, open = 0, content = 0;
+};
+
+VPT_HD void pa_tag_step(PaTagRun& r, bool start, uint32_t cls, uint32_t pos) {
+    if (start) r.start = pos + 1;
+    if (cls == kPaTagOpen) r.open = pos + 1;
+    if (cls == kPaTagContent) r.content = pos + 1;
+}
+
+VPT_HD void pa_tag_max(PaTagRun& r, const PaTagRun& o) {
+    r.start = r.start > o.start ? r.start : o.start;
+    r.open = r.open > o.open ? r.open : o.open;
+    r.content = r.content > o.content ? r.content : o.content;
+}
+
+// The written region of the current character: its first byte in the line and its length up to and including its last
+// content byte; length 0 when the character opened no region or its region holds no content (its fields are all empty)
+VPT_HD uint32_t pa_tag_region(const PaTagRun& r, uint32_t& first) {
+    first = r.open ? r.open - 1 : 0;
+    return r.open > r.start && r.content > r.open ? r.content - r.open + 1 : 0u;
+}
+
 }  // namespace vpt
