@@ -224,7 +224,10 @@ int vpt_predict(const vpt_predictor* predictor, const uint8_t* utf8, size_t n_by
  * maximum, predictor.rs:286-304) run in one kernel, k_tags; tokens of any length are served.  *d_unserved (nullable,
  * zero it first) counts tokens whose own tag model exceeds the limits of the device tables (more than 64 scores or 8 tag
  * slots; none of the reference's models): their entries are -1 and vpt_fill_tags serves them.  Returns VPT_UNSUPPORTED when the whole model is beyond
- * the limits, VPT_INVALID_ARGUMENT for a predictor created with predict_tags = false (the reference panics). */
+ * the limits, VPT_INVALID_ARGUMENT for a predictor created with predict_tags = false (the reference panics).
+ * d_utf8 must be 16-byte aligned and its allocation readable up to the next multiple of 16 bytes, as for
+ * vpt_predict_batch_dev.  d_boundaries holds 0 / 1 per pair of adjacent characters, as vpt_predict_batch_dev writes
+ * them; a caller may set its own 0 / 1 boundaries there to have the tags of that segmentation predicted. */
 int vpt_predict_tags_batch_dev(const vpt_predictor* predictor, const uint8_t* d_utf8, const uint64_t* d_byte_offsets,
                                size_t n_sent, const int32_t* d_status, const uint8_t* d_boundaries,
                                const uint64_t* d_bound_offsets, const uint64_t* d_char_offsets,

@@ -2511,6 +2511,8 @@ int vpt_predict_tags_batch_dev(const vpt_predictor* p, const uint8_t* d_utf8, co
         throw Error(kUnsupported, "this tag model exceeds the limits of the device path (tags.hpp); use vpt_fill_tags");
     if (!d_utf8 || !d_byte_offsets || !d_status || !d_boundaries || !d_bound_offsets || !d_char_offsets || !d_tag_token || !d_tag_cand)
         throw Error(kInvalidArgument, "InvalidArgumentError: device buffers: must not be NULL");
+    if (reinterpret_cast<uintptr_t>(d_utf8) & 15)
+        throw Error(kInvalidArgument, "InvalidArgumentError: d_utf8: must be 16-byte aligned");
     if ((p->dt.char_rels && !d_char_states) || (p->dt.type_rels && !d_type_states))
         throw Error(kInvalidArgument, "InvalidArgumentError: states: required for tag prediction");
     TagArgs t;
