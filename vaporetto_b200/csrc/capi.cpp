@@ -44,90 +44,117 @@ void cuda_check(cudaError_t e, const char* what) {
         throw Error(kCudaError, std::string("CUDA error in ") + what + ": " + cudaGetErrorString(e));
 }
 
-// Per-call scratch: a stream plus grow-only device buffers.
+// A grow-only device buffer of T, freed with its owner
+template <class T>
+class DevBuf {
+public:
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p_) cudaFree(p_); }
+    // At least `need` bytes, with an eighth and 256 bytes to spare when it grows.  The old buffer is freed before the
+    // new one is allocated (the peak is the new size alone); a failed allocation leaves the buffer empty.
+    T* ensure(size_t need) {
+        if (need <= cap_) return p_;
+        if (p_) cudaFree(p_);
+        p_ = nullptr;
+        cap_ = 0;
+        const size_t want = align_up(need + need / 8 + 256, 256);
+        cuda_check(cudaMalloc(&p_, want), "cudaMalloc(scratch)");
+        cap_ = want;
+        return p_;
+    }
+    T* get() const { return p_; }
+    size_t capacity() const { return cap_; }  // bytes
+
+private:
+    T* p_ = nullptr;
+    size_t cap_ = 0;
+};
+
+struct CudaFreeHost {
+    void operator()(void* q) const { cudaFreeHost(q); }
+};
+struct CudaFree {
+    void operator()(void* q) const { cudaFree(q); }
+};
+
+// The words a chunk's kernels and copies hand back to the host, in one pinned block per scratch
+struct HostTotals {
+    uint64_t bounds_chars[2];  // boundaries and characters of the count pass (BatchArgs::totals_host, written as a pair)
+    uint64_t lines;            // lines of the split pass (SplitArgs::n_lines_host)
+    uint64_t out_bytes;        // output bytes of a line chunk: the tokenized writer's, or dump_stage's with score dumps
+    uint64_t tokens;           // tokens of the compact and span passes (tok_total_host)
+    uint64_t tok_line_bytes;   // score dumps: the token line bytes the tokenized writer put in `stage`
+    uint64_t rule_suffix;      // the matched rules' suffix bytes, copied from the front of `trule`
+    uint64_t tag_scores;       // tag candidate scores of a chunk (TagScoreArgs::total_host)
+    uint64_t dump[2];          // score dumps: dump bytes, token line bytes (DumpArgs::total_host, written as a pair)
+    uint64_t eval[kEvalTotals + 1];  // evaluate: the chunk's totals, then the error key (also the partial parse's)
+};
+
+// Per-call scratch: two streams, grow-only device buffers and the pinned words the kernels write back.
 struct Scratch {
     cudaStream_t stream = nullptr;      // copy-in + kernels
     cudaStream_t stream_out = nullptr;  // copy-out: a chunk's D2H never delays the next chunk's H2D on `stream`
     cudaEvent_t ev_kernels = nullptr;   // recorded on `stream` after a chunk's last kernel
     cudaEvent_t ev_out = nullptr;       // recorded on `stream_out` after a chunk's last D2H copy
-    void* d_text = nullptr; size_t text_cap = 0;
-    void* d_off = nullptr; size_t off_cap = 0;
-    void* d_ws = nullptr; size_t ws_cap = 0;
-    void* d_status = nullptr; size_t status_cap = 0;
-    void* d_boff = nullptr; size_t boff_cap = 0;
-    void* d_coff = nullptr; size_t coff_cap = 0;
-    void* d_scores = nullptr; size_t scores_cap = 0;
-    void* d_bounds = nullptr; size_t bounds_cap = 0;
-    void* d_cst = nullptr; size_t cst_cap = 0;
-    void* d_tst = nullptr; size_t tst_cap = 0;
+    DevBuf<uint8_t> text;
+    DevBuf<uint64_t> off;
+    DevBuf<uint8_t> ws;                 // the scoring workspace, laid out by bind_workspace
+    DevBuf<int32_t> status;
+    DevBuf<uint64_t> boff;
+    DevBuf<uint64_t> coff;
+    DevBuf<int32_t> scores;
+    DevBuf<uint8_t> bounds;
+    DevBuf<uint32_t> cst;
+    DevBuf<uint32_t> tst;
     // line splitting / tokenised output (vpt_tokenize_lines)
-    void* d_trims = nullptr; size_t trims_cap = 0;
-    void* d_blk = nullptr; size_t blk_cap = 0;
-    void* d_blkbase = nullptr; size_t blkbase_cap = 0;
-    void* d_tokg = nullptr; size_t tokg_cap = 0;
-    void* d_out = nullptr; size_t out_cap = 0;
-    void* d_tok = nullptr; size_t tok_cap = 0;     // tag prediction outputs (vpt_predict_batch_tags)
-    void* d_cand = nullptr; size_t cand_cap = 0;
-    void* d_bits = nullptr; size_t bits_cap = 0;   // compact outputs (vpt_predict_batch_compact)
-    void* d_st8 = nullptr; size_t st8_cap = 0;
-    void* d_ntok = nullptr; size_t ntok_cap = 0;
-    void* d_tokbase = nullptr; size_t tokbase_cap = 0;
-    void* d_tokdesc = nullptr; size_t tokdesc_cap = 0;
-    void* d_tokwork = nullptr; size_t tokwork_cap = 0;  // work list of the per-token tag kernels (TagArgs::tok_work)
-    void* d_toklocal = nullptr; size_t toklocal_cap = 0;
-    void* d_tokblk = nullptr; size_t tokblk_cap = 0;
-    void* d_ends = nullptr; size_t ends_cap = 0;   // token byte ends (vpt_token_spans)
-    void* d_trule = nullptr; size_t trule_cap = 0; // tag rules: the matched suffix sum (8 bytes), then a rule id per token
-    void* d_scoff = nullptr; size_t scoff_cap = 0; // tag candidate scores (TagScoreArgs): per-record counts / offsets,
-    void* d_scblk = nullptr; size_t scblk_cap = 0; // block totals / prefix,
-    void* d_tagsc = nullptr; size_t tagsc_cap = 0; // the chunk's score vectors
+    DevBuf<uint8_t> trims;
+    DevBuf<uint32_t> blk;
+    DevBuf<uint64_t> blkbase;
+    DevBuf<uint64_t> tokg;              // look-back state words, then a u32 ticket
+    DevBuf<uint8_t> out;
+    DevBuf<int32_t> tok;                // tag prediction outputs (vpt_predict_batch_tags)
+    DevBuf<uint8_t> cand;               // u8 per token record; vpt_predict_batch_tags: i32 per character
+    DevBuf<uint32_t> bits;              // compact outputs (vpt_predict_batch_compact)
+    DevBuf<uint8_t> st8;
+    DevBuf<uint32_t> ntok;
+    DevBuf<uint64_t> tokbase;
+    DevBuf<uint4> tokdesc;
+    DevBuf<uint32_t> tokwork;           // work list of the per-token tag kernels (TagArgs::tok_work)
+    DevBuf<uint32_t> toklocal;
+    DevBuf<uint64_t> tokblk;
+    DevBuf<uint32_t> ends;              // token byte ends (vpt_token_spans)
+    DevBuf<unsigned long long> trule;   // tag rules: the matched suffix sum (8 bytes), then a rule id per token
+    DevBuf<uint32_t> scoff;             // tag candidate scores (TagScoreArgs): per-record counts / offsets,
+    DevBuf<uint64_t> scblk;             // block totals / prefix,
+    DevBuf<int32_t> tagsc;              // the chunk's score vectors
     // score dumps of the lines path (dump.hpp): the token lines in front of their dumps, the per-line sizes
-    void* d_stage = nullptr; size_t stage_cap = 0;
-    void* d_dsize = nullptr; size_t dsize_cap = 0;
+    DevBuf<uint8_t> stage;
+    DevBuf<uint64_t> dsize;
     // gold corpus and metrics (vpt_evaluate_lines); the partial parse (vpt_tokenize_partial_lines) uses gtext, goff,
     // gcoff, gbnd (its marker codes) and evtot (its error key); vpt_annotate_lines keeps its output markers in gbnd,
     // vpt_reannotate_lines in pmark (gbnd holds the input's), and its input tag regions in ptag
-    void* d_gtext = nullptr; size_t gtext_cap = 0;
-    void* d_goff = nullptr; size_t goff_cap = 0;
-    void* d_gcoff = nullptr; size_t gcoff_cap = 0;
-    void* d_gbnd = nullptr; size_t gbnd_cap = 0;
-    void* d_gtag = nullptr; size_t gtag_cap = 0;
-    void* d_gw = nullptr; size_t gw_cap = 0;
-    void* d_lc = nullptr; size_t lc_cap = 0;
-    void* d_evtot = nullptr; size_t evtot_cap = 0;
-    void* d_pmark = nullptr; size_t pmark_cap = 0;
-    void* d_ptag = nullptr; size_t ptag_cap = 0;
-    uint64_t* h_eval = nullptr;    // pinned, kEvalTotals + 1 x u64: a chunk's totals and error key
-    uint64_t* h_totals = nullptr;  // pinned, 10 x u64: boundaries, chars, lines, output bytes, tokens (score dumps: the
-                                   // writer's token line bytes), first bit word, rule suffix bytes, tag scores, then the
-                                   // score dumps' dump bytes and token line bytes
-    uint32_t* h_side = nullptr; size_t side_cap = 0;  // pinned: first bit word of every chunk (vpt_predict_batch_compact)
-    uint8_t* h_io = nullptr;       // pinned staging of the single-sentence call (vpt_predict), kSingleIoBytes
-    void* d_io = nullptr;          // its device twin
+    DevBuf<uint8_t> gtext;
+    DevBuf<uint64_t> goff;
+    DevBuf<uint64_t> gcoff;
+    DevBuf<uint8_t> gbnd;
+    DevBuf<uint32_t> gtag;
+    DevBuf<uint32_t> gw;
+    DevBuf<uint32_t> lc;
+    DevBuf<uint64_t> evtot;
+    DevBuf<uint8_t> pmark;
+    DevBuf<uint2> ptag;
+    std::unique_ptr<HostTotals, CudaFreeHost> totals;  // pinned, allocated with the scratch (ScratchLease)
+    std::unique_ptr<uint32_t[], CudaFreeHost> h_side;  // pinned: first bit word of every chunk (vpt_predict_batch_compact)
+    size_t side_words = 0;                             // words of h_side
+    std::unique_ptr<uint8_t[], CudaFreeHost> h_io;     // pinned staging of the single-sentence call (vpt_predict), kSingleIoBytes
+    std::unique_ptr<uint8_t[], CudaFree> d_io;         // its device twin
     ~Scratch() {
-        for (void* p : {d_text, d_off, d_ws, d_status, d_boff, d_coff, d_scores, d_bounds, d_cst, d_tst, d_trims, d_blk,
-                        d_blkbase, d_tokg, d_out, d_tok, d_cand, d_bits, d_st8, d_ntok, d_tokbase, d_tokdesc, d_tokwork, d_toklocal, d_tokblk, d_ends, d_trule,
-                        d_scoff, d_scblk, d_tagsc, d_stage, d_dsize,
-                        d_gtext, d_goff, d_gcoff, d_gbnd, d_gtag, d_gw, d_lc, d_evtot, d_pmark, d_ptag})
-            if (p) cudaFree(p);
-        if (h_totals) cudaFreeHost(h_totals);
-        if (h_eval) cudaFreeHost(h_eval);
-        if (h_io) cudaFreeHost(h_io);
-        if (h_side) cudaFreeHost(h_side);
-        if (d_io) cudaFree(d_io);
         if (ev_kernels) cudaEventDestroy(ev_kernels);
         if (ev_out) cudaEventDestroy(ev_out);
         if (stream_out) cudaStreamDestroy(stream_out);
         if (stream) cudaStreamDestroy(stream);
-    }
-    static void ensure(void*& p, size_t& cap, size_t need) {
-        if (need <= cap) return;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = align_up(need + need / 8 + 256, 256);
-        cuda_check(cudaMalloc(&p, want), "cudaMalloc(scratch)");
-        cap = want;
     }
 };
 
@@ -351,7 +378,9 @@ struct ScratchLease {
             cuda_check(cudaStreamCreateWithFlags(&s->stream_out, cudaStreamNonBlocking), "cudaStreamCreate");
             cuda_check(cudaEventCreateWithFlags(&s->ev_kernels, cudaEventDisableTiming), "cudaEventCreate");
             cuda_check(cudaEventCreateWithFlags(&s->ev_out, cudaEventDisableTiming), "cudaEventCreate");
-            cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s->h_totals), 80), "cudaMallocHost");
+            HostTotals* h = nullptr;
+            cuda_check(cudaMallocHost(reinterpret_cast<void**>(&h), sizeof(HostTotals)), "cudaMallocHost");
+            s->totals.reset(h);
         }
     }
     ~ScratchLease() {
@@ -415,14 +444,10 @@ TagArgs tag_args(const DevTags& dt, const BatchArgs& a) {
 // max_tokens) into `r`, a TagArgs or a SpanStage
 template <class R>
 void bind_token_records(const vpt_predictor& p, Scratch& s, R& r, uint64_t m) {
-    Scratch::ensure(s.d_tok, s.tok_cap, 4 * m + 16);
-    Scratch::ensure(s.d_cand, s.cand_cap, m * std::max<size_t>(p.n_tags, 1) + 16);
-    Scratch::ensure(s.d_tokdesc, s.tokdesc_cap, 16 * m + 16);
-    Scratch::ensure(s.d_tokwork, s.tokwork_cap, 4 * m + 32);
-    r.tok_ids = static_cast<int32_t*>(s.d_tok);
-    r.tok_cands = static_cast<uint8_t*>(s.d_cand);
-    r.tok_desc = static_cast<uint4*>(s.d_tokdesc);
-    r.tok_work = static_cast<uint32_t*>(s.d_tokwork);
+    r.tok_ids = s.tok.ensure(4 * m + 16);
+    r.tok_cands = s.cand.ensure(m * std::max<size_t>(p.n_tags, 1) + 16);
+    r.tok_desc = s.tokdesc.ensure(16 * m + 16);
+    r.tok_work = s.tokwork.ensure(4 * m + 32);
     r.max_tokens = m;
 }
 
@@ -430,14 +455,10 @@ void bind_token_records(const vpt_predictor& p, Scratch& s, R& r, uint64_t m) {
 // tok_blk) into `k`, a CompactArgs or a SpanStage; the prefix of both kernels runs in blocks of kSpanDocs sentences
 template <class K>
 void bind_token_counts(Scratch& s, K& k, size_t n) {
-    Scratch::ensure(s.d_ntok, s.ntok_cap, 4 * n + 16);
-    Scratch::ensure(s.d_tokbase, s.tokbase_cap, 8 * (n + 1) + 16);
-    Scratch::ensure(s.d_toklocal, s.toklocal_cap, 4 * n + 16);
-    Scratch::ensure(s.d_tokblk, s.tokblk_cap, 8 * (n / kSpanDocs + 4));
-    k.n_tokens = static_cast<uint32_t*>(s.d_ntok);
-    k.tok_base = static_cast<uint64_t*>(s.d_tokbase);
-    k.tok_local = static_cast<uint32_t*>(s.d_toklocal);
-    k.tok_blk = static_cast<uint64_t*>(s.d_tokblk);
+    k.n_tokens = s.ntok.ensure(4 * n + 16);
+    k.tok_base = s.tokbase.ensure(8 * (n + 1) + 16);
+    k.tok_local = s.toklocal.ensure(4 * n + 16);
+    k.tok_blk = s.tokblk.ensure(8 * (n / kSpanDocs + 4));
 }
 
 // ---- host-side text helpers ------------------------------------------------------------------------
@@ -920,32 +941,27 @@ void chunk_count(Scratch& s, ChunkState& ch, const uint8_t* utf8, const uint64_t
     cudaStream_t st = s.stream;
     const WorkspaceLayout wl = workspace_layout(ch.n);
     const size_t shift = size_t(ch.byte_lo & 15);
-    Scratch::ensure(s.d_text, s.text_cap, shift + ch.nbytes + 64);
-    Scratch::ensure(s.d_off, s.off_cap, 8 * (ch.n + 1));
-    Scratch::ensure(s.d_ws, s.ws_cap, wl.total);
-    Scratch::ensure(s.d_status, s.status_cap, 4 * ch.n);
-    Scratch::ensure(s.d_boff, s.boff_cap, 8 * (ch.n + 1));
-    Scratch::ensure(s.d_coff, s.coff_cap, 8 * (ch.n + 1));
+    BatchArgs& a = ch.a;
+    a = BatchArgs();
+    uint8_t* const text = s.text.ensure(shift + ch.nbytes + 64);
+    uint64_t* const offsets = s.off.ensure(8 * (ch.n + 1));
+    bind_workspace(a, s.ws.ensure(wl.total), ch.n);
+    a.status = s.status.ensure(4 * ch.n);
+    a.bound_offsets = s.boff.ensure(8 * (ch.n + 1));
+    a.char_offsets = s.coff.ensure(8 * (ch.n + 1));
     if (ch.nbytes)
-        cuda_check(cudaMemcpyAsync(static_cast<uint8_t*>(s.d_text) + shift, utf8 + ch.byte_lo, ch.nbytes,
-                                   cudaMemcpyHostToDevice, st), "H2D(text)");
-    cuda_check(cudaMemcpyAsync(s.d_off, byte_offsets + ch.s_lo, 8 * (ch.n + 1), cudaMemcpyHostToDevice, st), "H2D(offsets)");
+        cuda_check(cudaMemcpyAsync(text + shift, utf8 + ch.byte_lo, ch.nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
+    cuda_check(cudaMemcpyAsync(offsets, byte_offsets + ch.s_lo, 8 * (ch.n + 1), cudaMemcpyHostToDevice, st), "H2D(offsets)");
     // the kernels overwrite buffers the previous chunk of this scratch may still be copying out
     cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
     if (pipeline_trace()) ch.tr.mark(0, st);
-    BatchArgs& a = ch.a;
-    a = BatchArgs();
     // offsets are absolute in the caller's buffer: bias the text pointer so that text[offset] is right
-    a.text = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(s.d_text) + shift - uintptr_t(ch.byte_lo));
-    a.offsets = static_cast<const uint64_t*>(s.d_off);
+    a.text = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(text) + shift - uintptr_t(ch.byte_lo));
+    a.offsets = offsets;
     a.n_sent = ch.n;
-    bind_workspace(a, s.d_ws, ch.n);
-    a.status = static_cast<int32_t*>(s.d_status);
-    a.bound_offsets = static_cast<uint64_t*>(s.d_boff);
-    a.char_offsets = static_cast<uint64_t*>(s.d_coff);
     // the totals come back through pinned host memory the scan kernel writes itself: an 8-byte D2H copy would
     // queue behind the bulk copy-out of earlier chunks on the copy engine
-    a.totals_host = &s.h_totals[0];
+    a.totals_host = s.totals->bounds_chars;
     cuda_check(launch_count(a, st), "launch(count)");
     if (!ch.counted) cuda_check(cudaEventCreateWithFlags(&ch.counted, cudaEventDisableTiming), "cudaEventCreate");
     cuda_check(cudaEventRecord(ch.counted, st), "cudaEventRecord");
@@ -1008,8 +1024,8 @@ struct BatchRing {
                 ChunkState& ch = chunks[step];
                 Scratch& s = scratch(step);
                 cuda_check(cudaEventSynchronize(ch.counted), "sync(count)");
-                ch.nb = s.h_totals[0];
-                ch.nc = s.h_totals[1];
+                ch.nb = s.totals->bounds_chars[0];
+                ch.nc = s.totals->bounds_chars[1];
                 ch.issued = issue(step, ch, s);
                 if (ch.issued) {
                     if (trace) ch.tr.mark(2, s.stream);
@@ -1076,15 +1092,11 @@ int vpt_predict_batch(const vpt_predictor* p, const uint8_t* utf8, const uint64_
         nb_total += nb;
         nc_total += nc;
         if (overflow) return false;
-        Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
+        a.boundaries = s.bounds.ensure(nb + 4);
         a.scores = nullptr;  // boundaries only, when the caller wants no scores and the kernel can skip them
-        if (scores_out || !scores_optional(p->dm)) {
-            Scratch::ensure(s.d_scores, s.scores_cap, 4 * nb + 4);
-            a.scores = static_cast<int32_t*>(s.d_scores);
-        }
-        a.boundaries = static_cast<uint8_t*>(s.d_bounds);
-        if (char_states_out) { Scratch::ensure(s.d_cst, s.cst_cap, 4 * nc + 4); a.char_states = static_cast<uint32_t*>(s.d_cst); }
-        if (type_states_out) { Scratch::ensure(s.d_tst, s.tst_cap, 4 * nc + 4); a.type_states = static_cast<uint32_t*>(s.d_tst); }
+        if (scores_out || !scores_optional(p->dm)) a.scores = s.scores.ensure(4 * nb + 4);
+        if (char_states_out) a.char_states = s.cst.ensure(4 * nc + 4);
+        if (type_states_out) a.type_states = s.tst.ensure(4 * nc + 4);
         if (pipeline_trace()) ch.tr.mark(1, st);
         cuda_check(launch_score(p->dm, a, st), "launch(score)");
         return true;
@@ -1092,17 +1104,17 @@ int vpt_predict_batch(const vpt_predictor* p, const uint8_t* utf8, const uint64_
     auto copy_out = [&](size_t c, ChunkState& ch, Scratch& s, cudaStream_t so) {
         const uint64_t nb = ch.nb, nc = ch.nc, b0 = ch.a.bound_base, c0 = ch.a.char_base;
         if (nb) {
-            if (scores_out) cuda_check(cudaMemcpyAsync(scores_out + b0, s.d_scores, 4 * nb, cudaMemcpyDeviceToHost, so), "D2H(scores)");
-            cuda_check(cudaMemcpyAsync(boundaries_out + b0, s.d_bounds, nb, cudaMemcpyDeviceToHost, so), "D2H(boundaries)");
+            if (scores_out) cuda_check(cudaMemcpyAsync(scores_out + b0, s.scores.get(), 4 * nb, cudaMemcpyDeviceToHost, so), "D2H(scores)");
+            cuda_check(cudaMemcpyAsync(boundaries_out + b0, s.bounds.get(), nb, cudaMemcpyDeviceToHost, so), "D2H(boundaries)");
         }
         // the last element of a chunk's offsets is the first of the next chunk's: copy n (+1 for the last chunk)
         const size_t noff = ch.n + (c + 1 == nchunks ? 1 : 0);
-        cuda_check(cudaMemcpyAsync(bound_offsets_out + ch.s_lo, s.d_boff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
+        cuda_check(cudaMemcpyAsync(bound_offsets_out + ch.s_lo, s.boff.get(), 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
         if (char_offsets_out)
-            cuda_check(cudaMemcpyAsync(char_offsets_out + ch.s_lo, s.d_coff, 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
-        if (status_out) cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_status, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
-        if (nc && char_states_out) cuda_check(cudaMemcpyAsync(char_states_out + c0, s.d_cst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
-        if (nc && type_states_out) cuda_check(cudaMemcpyAsync(type_states_out + c0, s.d_tst, 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
+            cuda_check(cudaMemcpyAsync(char_offsets_out + ch.s_lo, s.coff.get(), 8 * noff, cudaMemcpyDeviceToHost, so), "D2H(offsets)");
+        if (status_out) cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.status.get(), 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
+        if (nc && char_states_out) cuda_check(cudaMemcpyAsync(char_states_out + c0, s.cst.get(), 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
+        if (nc && type_states_out) cuda_check(cudaMemcpyAsync(type_states_out + c0, s.tst.get(), 4 * nc, cudaMemcpyDeviceToHost, so), "D2H(states)");
     };
     ring.run(utf8, byte_offsets, false, issue, copy_out);
     if (n_boundaries_out) *n_boundaries_out = nb_total;
@@ -1152,19 +1164,17 @@ struct LineJob {
 void lines_stage0(Scratch& s, LineChunk& ch, const uint8_t* bytes) {
     cudaStream_t st = s.stream;
     const size_t nblk = (ch.nbytes + kSplitBlockBytes - 1) / kSplitBlockBytes;
-    Scratch::ensure(s.d_text, s.text_cap, ch.nbytes + 64);
-    Scratch::ensure(s.d_blk, s.blk_cap, 4 * nblk + 4);
-    Scratch::ensure(s.d_blkbase, s.blkbase_cap, 8 * nblk + 16);
-    cuda_check(cudaMemcpyAsync(s.d_text, bytes, ch.nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
-    if (pipeline_trace()) ch.tr.mark(0, st);
     SplitArgs& sp = ch.sp;
     sp = SplitArgs();
-    sp.text = static_cast<const uint8_t*>(s.d_text);
+    uint8_t* const text = s.text.ensure(ch.nbytes + 64);
+    sp.blk = s.blk.ensure(4 * nblk + 4);
+    sp.blk_base = s.blkbase.ensure(8 * nblk + 16);
+    cuda_check(cudaMemcpyAsync(text, bytes, ch.nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
+    if (pipeline_trace()) ch.tr.mark(0, st);
+    sp.text = text;
     sp.n_bytes = ch.nbytes;
-    sp.blk = static_cast<uint32_t*>(s.d_blk);
-    sp.blk_base = static_cast<uint64_t*>(s.d_blkbase);
     sp.n_lines = sp.blk_base + nblk;  // the element after the per-block bases
-    sp.n_lines_host = &s.h_totals[2];  // read back through pinned host memory written by the kernel (see chunk_count)
+    sp.n_lines_host = &s.totals->lines;  // read back through pinned host memory written by the kernel (see chunk_count)
     cuda_check(launch_split_count(sp, st), "launch(split)");
     if (!ch.split) cuda_check(cudaEventCreateWithFlags(&ch.split, cudaEventDisableTiming), "cudaEventCreate");
     cuda_check(cudaEventRecord(ch.split, st), "cudaEventRecord");
@@ -1249,30 +1259,21 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     cudaStream_t st = s.stream;
     const size_t n = size_t(a.n_sent);
     const WorkspaceLayout wl = workspace_layout(n);
-    Scratch::ensure(s.d_ws, s.ws_cap, wl.total);
-    Scratch::ensure(s.d_status, s.status_cap, 4 * n);
-    Scratch::ensure(s.d_boff, s.boff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_bounds, s.bounds_cap, nbytes + 4);
-    bind_workspace(a, s.d_ws, n);
-    a.status = static_cast<int32_t*>(s.d_status);
-    a.bound_offsets = static_cast<uint64_t*>(s.d_boff);
+    bind_workspace(a, s.ws.ensure(wl.total), n);
+    a.status = s.status.ensure(4 * n);
+    a.bound_offsets = s.boff.ensure(8 * (n + 1));
+    a.boundaries = s.bounds.ensure(nbytes + 4);
     // the callers need the boundaries only (every character is at least one byte: the bytes bound the boundaries)
     a.scores = nullptr;
     DevModel dm = p.dm;
     dm.kytea_norm = normalize ? 1 : 0;
-    if (!scores_optional(dm) || (job.dumps & kDumpScores) || (ann && ann->margin > 0)) {
-        Scratch::ensure(s.d_scores, s.scores_cap, 4 * nbytes + 4);
-        a.scores = static_cast<int32_t*>(s.d_scores);
-    }
-    a.boundaries = static_cast<uint8_t*>(s.d_bounds);
+    if (!scores_optional(dm) || (job.dumps & kDumpScores) || (ann && ann->margin > 0))
+        a.scores = s.scores.ensure(4 * nbytes + 4);
     if (tags) {
         // tag prediction needs the pattern-id states and the character offsets of the sentences
-        Scratch::ensure(s.d_cst, s.cst_cap, 4 * nbytes + 16);
-        Scratch::ensure(s.d_tst, s.tst_cap, 4 * nbytes + 16);
-        Scratch::ensure(s.d_coff, s.coff_cap, 8 * (n + 1));
-        a.char_states = static_cast<uint32_t*>(s.d_cst);
-        a.type_states = static_cast<uint32_t*>(s.d_tst);
-        a.char_offsets = static_cast<uint64_t*>(s.d_coff);
+        a.char_states = s.cst.ensure(4 * nbytes + 16);
+        a.type_states = s.tst.ensure(4 * nbytes + 16);
+        a.char_offsets = s.coff.ensure(8 * (n + 1));
     }
     if (pipeline_trace()) ch.tr.mark_sub(0, st);  // after the line offsets
     if (!fused_ok(dm)) cuda_check(launch_count(a, st), "launch(count)");
@@ -1309,8 +1310,7 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
     if (ann) cuda_check(launch_pa_marks(*ann, st), "launch(marks)");
     if (tags) {
         TagRecords r;
-        Scratch::ensure(s.d_st8, s.st8_cap, n + 16);
-        r.status8 = static_cast<uint8_t*>(s.d_st8);
+        r.status8 = s.st8.ensure(n + 16);
         bind_token_counts(s, r, n);
         bind_token_records(p, s, r, nbytes);
         if ((job.dumps & kDumpTagScores) && sc) {
@@ -1318,9 +1318,8 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
             r.scores = sc;
         }
         if (job.rules && ra) {
-            Scratch::ensure(s.d_trule, s.trule_cap, 4 * nbytes + 16);
             r.rules = job.rules;
-            r.rule_words = static_cast<unsigned long long*>(s.d_trule);
+            r.rule_words = s.trule.ensure(4 * nbytes + 16);
         }
         launch_tag_records(p, a, normalize, r, t, ra, st);
         if (ann) {
@@ -1338,17 +1337,15 @@ TokArgs predict_lines(const vpt_predictor& p, Scratch& s, LineChunk& ch, BatchAr
 size_t split_lines(Scratch& s, LineChunk& ch) {
     cudaStream_t st = s.stream;
     cuda_check(cudaEventSynchronize(ch.split), "sync(split)");
-    const size_t n = size_t(s.h_totals[2]);
+    const size_t n = size_t(s.totals->lines);
     ch.n_lines = n;
     if (!ch.done) cuda_check(cudaEventCreateWithFlags(&ch.done, cudaEventDisableTiming), "cudaEventCreate");
     if (n == 0) return 0;
     const size_t ng = (n + kGroup - 1) / kGroup;
-    Scratch::ensure(s.d_off, s.off_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_trims, s.trims_cap, n + 4);
-    Scratch::ensure(s.d_tokg, s.tokg_cap, 8 * (ng + 2));
-    ch.sp.offsets = static_cast<uint64_t*>(s.d_off);
-    ch.sp.trims = static_cast<uint8_t*>(s.d_trims);
-    // the kernels of the stage overwrite outputs (d_out, d_lc) the previous chunk of this scratch may still be copying out
+    ch.sp.offsets = s.off.ensure(8 * (n + 1));
+    ch.sp.trims = s.trims.ensure(n + 4);
+    s.tokg.ensure(8 * (ng + 2));  // the look-back state words and ticket of the stage's parse and writer
+    // the kernels of the stage overwrite outputs (out, lc) the previous chunk of this scratch may still be copying out
     cuda_check(cudaStreamWaitEvent(st, s.ev_out, 0), "cudaStreamWaitEvent");
     if (pipeline_trace()) ch.tr.mark(1, st);
     cuda_check(launch_split_write(ch.sp, st), "launch(split)");
@@ -1357,7 +1354,7 @@ size_t split_lines(Scratch& s, LineChunk& ch) {
 
 // The score dumps of a chunk (dump.hpp) behind its token lines, which `t` wrote to the staging buffer: every line's dump
 // bytes and token line bytes with their prefixes and totals, one wait for the totals, then the output, sized exactly,
-// with its size in h_totals[3].  The token lines are placed by their computed sizes, not by their '\n's: a tag string
+// with its size in `out_bytes`.  The token lines are placed by their computed sizes, not by their '\n's: a tag string
 // (of the model or of a rule) may hold a '\n'.
 void dump_stage(const vpt_predictor& p, Scratch& s, const TokArgs& t, const BatchArgs& a, const TagScoreArgs& sc,
                 const TagRuleArgs& ra, const LineJob& job) {
@@ -1388,54 +1385,50 @@ void dump_stage(const vpt_predictor& p, Scratch& s, const TokArgs& t, const Batc
         d.rules = ra.rules;
     }
     if (job.dumps & kDumpTagScores) {
-        d.tok_desc = static_cast<const uint4*>(s.d_tokdesc);
+        d.tok_desc = s.tokdesc.get();
         d.rec_off = sc.rec_off;
         d.score_blk = sc.blk;
         d.tag_scores = sc.scores;
         d.tok_info = p.dt.tok_info;
     }
     const size_t nblk = (n + kDumpBlock - 1) / kDumpBlock;
-    Scratch::ensure(s.d_dsize, s.dsize_cap, 8 * (3 * n + 2 * nblk + 4));
-    d.size = static_cast<uint64_t*>(s.d_dsize);
+    d.size = s.dsize.ensure(8 * (3 * n + 2 * nblk + 4));
     d.tl_len = d.size + n;
     d.tl_off = d.tl_len + n;
     d.blk = d.tl_off + n;
-    d.total_host = &s.h_totals[8];
+    d.total_host = s.totals->dump;
     cuda_check(launch_dump_size(d, st), "launch(dump size)");
     cuda_check(cudaStreamSynchronize(st), "sync(dump size)");
-    const uint64_t tok_bytes = s.h_totals[4], dump_bytes = s.h_totals[8];
+    const uint64_t tok_bytes = s.totals->tok_line_bytes, dump_bytes = s.totals->dump[0];
     // token_line_len restates the writers' sizes: a disagreement would misplace every later line of the chunk
-    if (s.h_totals[9] != tok_bytes)
-        throw Error(kInternal, "internal error: score dumps: token line sizes (" + std::to_string(s.h_totals[9]) +
+    if (s.totals->dump[1] != tok_bytes)
+        throw Error(kInternal, "internal error: score dumps: token line sizes (" + std::to_string(s.totals->dump[1]) +
                                    ") disagree with the writer's (" + std::to_string(tok_bytes) + ")");
-    Scratch::ensure(s.d_out, s.out_cap, tok_bytes + dump_bytes + 4);
-    d.tok_lines = static_cast<const uint8_t*>(s.d_stage);
-    d.out = static_cast<uint8_t*>(s.d_out);
+    d.out = s.out.ensure(tok_bytes + dump_bytes + 4);
+    d.tok_lines = s.stage.get();
     cuda_check(launch_dump_write(d, st), "launch(dump)");
-    s.h_totals[3] = tok_bytes - n + dump_bytes;  // dump_line writes each token line's '\n' itself
+    s.totals->out_bytes = tok_bytes - n + dump_bytes;  // dump_line writes each token line's '\n' itself
 }
 
 // stage 1: line offsets, count + score, tokenised bytes; the output size to pinned host memory
 void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
     cudaStream_t st = s.stream;
     const size_t n = split_lines(s, ch);
-    s.h_totals[3] = 0;
+    s.totals->out_bytes = 0;
     if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
     const size_t ng = (n + kGroup - 1) / kGroup;
     // with the score dumps the token lines go to a staging buffer, and the dump writer puts them in front of their dumps
-    void*& tok_buf = job.dumps ? s.d_stage : s.d_out;
-    size_t& tok_cap = job.dumps ? s.stage_cap : s.out_cap;
+    DevBuf<uint8_t>& tok_buf = job.dumps ? s.stage : s.out;
     // surface bytes + at most one '\\' per byte + at most one ' ' per character + one '\n' per line
     // (with tags: every token -- at most one per byte -- may get the longest "/tag/.." suffix of the model; the
     // partial-annotation format has one marker per character and no escapes, so the same bound holds for it)
     const size_t out_need = 3 * ch.nbytes + n + 4 + (job.tags ? size_t(ch.nbytes) * p.dt.max_suffix : 0);
-    Scratch::ensure(tok_buf, tok_cap, out_need);
+    tok_buf.ensure(out_need);
     const bool annotate = job.kind == kJobAnnotate;
     AnnArgs ann;
     if (annotate) {
-        Scratch::ensure(s.d_gbnd, s.gbnd_cap, ch.nbytes + 4);
         ann.margin = job.margin;
-        ann.marks = static_cast<uint8_t*>(s.d_gbnd);
+        ann.marks = s.gbnd.ensure(ch.nbytes + 4);
     }
     BatchArgs a;
     a.text = ch.sp.text;
@@ -1448,17 +1441,17 @@ void lines_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJ
     if (ra.tok_rule) {
         // A rule's tag may be long on a short surface, so the rules' share of the output is sized from the suffixes the
         // chunk's tokens actually matched: the host waits for the rule lookup and reads their sum.
-        cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
+        cuda_check(cudaMemcpyAsync(&s.totals->rule_suffix, s.trule.get(), 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
         cuda_check(cudaStreamSynchronize(st), "sync(rules)");
-        Scratch::ensure(tok_buf, tok_cap, out_need + size_t(s.h_totals[6]));
+        tok_buf.ensure(out_need + size_t(s.totals->rule_suffix));
         uint64_t seen = job.rules->max_out.load();
-        while (seen < tok_cap && !job.rules->max_out.compare_exchange_weak(seen, tok_cap)) {}
+        while (seen < tok_buf.capacity() && !job.rules->max_out.compare_exchange_weak(seen, tok_buf.capacity())) {}
     }
-    t.tok_state = static_cast<uint64_t*>(s.d_tokg);
+    t.tok_state = s.tokg.get();
     t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
     t.total = t.tok_state + ng + 1;
-    t.total_host = &s.h_totals[job.dumps ? 4 : 3];
-    t.out = static_cast<uint8_t*>(tok_buf);
+    t.total_host = job.dumps ? &s.totals->tok_line_bytes : &s.totals->out_bytes;
+    t.out = tok_buf.get();
     if (annotate) cuda_check(launch_pa_write(t, ra, ann.marks, st), "launch(annotate)");
     else cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
     if (job.dumps) dump_stage(p, s, t, a, sc, ra, job);
@@ -1533,39 +1526,31 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
                  uint64_t line_lo) {
     cudaStream_t st = s.stream;
     const size_t n = split_lines(s, ch);
-    if (!s.h_eval) cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s.h_eval), 8 * (kEvalTotals + 1)), "cudaMallocHost");
     if (n == 0) {
-        for (int i = 0; i < kEvalTotals; ++i) s.h_eval[i] = 0;
-        s.h_eval[kEvalTotals] = kGoldNoError;
+        for (int i = 0; i < kEvalTotals; ++i) s.totals->eval[i] = 0;
+        s.totals->eval[kEvalTotals] = kGoldNoError;
         cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
         return;
     }
     const size_t ng = (n + kGroup - 1) / kGroup;
     const size_t nb = ch.nbytes;  // bounds the surface bytes and characters of the chunk
     const int tag_mode = job.tag_mode;
-    Scratch::ensure(s.d_gtext, s.gtext_cap, nb + 64);
-    Scratch::ensure(s.d_goff, s.goff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_gbnd, s.gbnd_cap, nb + 4);
-    Scratch::ensure(s.d_gw, s.gw_cap, 4 * n + 4);
-    Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
-    if (tag_mode == kTagsCompare) Scratch::ensure(s.d_gtag, s.gtag_cap, 4 * nb + 4);
-    if (line_counts) Scratch::ensure(s.d_lc, s.lc_cap, 28 * n + 4);
     EvalArgs e;
     e.text = ch.sp.text;
     e.offsets = ch.sp.offsets;
     e.trims = ch.sp.trims;
     e.n_sent = n;
-    e.surface = static_cast<uint8_t*>(s.d_gtext);
-    e.surf_offsets = static_cast<uint64_t*>(s.d_goff);
-    e.char_offsets = static_cast<uint64_t*>(s.d_gcoff);
-    e.gold_bnd = static_cast<uint8_t*>(s.d_gbnd);
-    e.tag_pos = tag_mode == kTagsCompare ? static_cast<uint32_t*>(s.d_gtag) : nullptr;
-    e.width = static_cast<uint32_t*>(s.d_gw);
-    e.state = static_cast<uint64_t*>(s.d_tokg);
-    e.ticket = reinterpret_cast<uint32_t*>(e.state + ng);
-    e.totals = static_cast<uint64_t*>(s.d_evtot);
+    e.surface = s.gtext.ensure(nb + 64);
+    e.surf_offsets = s.goff.ensure(8 * (n + 1));
+    e.char_offsets = s.gcoff.ensure(8 * (n + 1));
+    e.gold_bnd = s.gbnd.ensure(nb + 4);
+    e.width = s.gw.ensure(4 * n + 4);
+    e.totals = s.evtot.ensure(8 * (kEvalTotals + 1));
     e.err = e.totals + kEvalTotals;
+    e.tag_pos = tag_mode == kTagsCompare ? s.gtag.ensure(4 * nb + 4) : nullptr;
+    e.line_counts = line_counts ? s.lc.ensure(28 * n + 4) : nullptr;
+    e.state = s.tokg.get();
+    e.ticket = reinterpret_cast<uint32_t*>(e.state + ng);
     cuda_check(cudaMemsetAsync(e.totals, 0, 8 * kEvalTotals, st), "cudaMemset");
     cuda_check(cudaMemsetAsync(e.err, 0xFF, 8, st), "cudaMemset");
     cuda_check(launch_gold_parse(e, st), "launch(gold)");
@@ -1589,15 +1574,14 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
         e.ts_ref = t.ts_ref;
         e.ts_bytes = t.ts_bytes;
     }
-    e.line_counts = line_counts ? static_cast<uint32_t*>(s.d_lc) : nullptr;
     cuda_check(launch_eval(e, st), "launch(eval)");
-    cuda_check(cudaMemcpyAsync(s.h_eval, e.totals, 8 * (kEvalTotals + 1), cudaMemcpyDeviceToHost, st), "D2H(totals)");
+    cuda_check(cudaMemcpyAsync(s.totals->eval, e.totals, 8 * (kEvalTotals + 1), cudaMemcpyDeviceToHost, st), "D2H(totals)");
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
     if (line_counts) {
         cuda_check(cudaEventRecord(s.ev_kernels, st), "cudaEventRecord");
         cuda_check(cudaStreamWaitEvent(s.stream_out, s.ev_kernels, 0), "cudaStreamWaitEvent");
-        cuda_check(cudaMemcpyAsync(line_counts + 7 * line_lo, s.d_lc, 28 * n, cudaMemcpyDeviceToHost, s.stream_out), "D2H(counts)");
+        cuda_check(cudaMemcpyAsync(line_counts + 7 * line_lo, s.lc.get(), 28 * n, cudaMemcpyDeviceToHost, s.stream_out), "D2H(counts)");
         cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
     }
 }
@@ -1610,17 +1594,17 @@ void eval_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
 void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJob& job) {
     cudaStream_t st = s.stream;
     const size_t n = split_lines(s, ch);
-    if (!s.h_eval) cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s.h_eval), 8 * (kEvalTotals + 1)), "cudaMallocHost");
-    s.h_totals[3] = 0;
-    s.h_eval[kEvalTotals] = kGoldNoError;
+    s.totals->out_bytes = 0;
+    s.totals->eval[kEvalTotals] = kGoldNoError;
     if (n == 0) { cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord"); return; }
     const size_t ng = (n + kGroup - 1) / kGroup;
     const size_t nb = ch.nbytes;  // bounds the raw bytes, the characters and the markers of the chunk
-    Scratch::ensure(s.d_gtext, s.gtext_cap, nb + 64);
-    Scratch::ensure(s.d_goff, s.goff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_gcoff, s.gcoff_cap, 8 * (n + 1));
-    Scratch::ensure(s.d_gbnd, s.gbnd_cap, nb + 4);
-    Scratch::ensure(s.d_evtot, s.evtot_cap, 8 * (kEvalTotals + 1));
+    PartArgs e;
+    e.surface = s.gtext.ensure(nb + 64);
+    e.surf_offsets = s.goff.ensure(8 * (n + 1));
+    e.char_offsets = s.gcoff.ensure(8 * (n + 1));
+    e.given = s.gbnd.ensure(nb + 4);
+    e.err = s.evtot.ensure(8 * (kEvalTotals + 1)) + kEvalTotals;
     // as lines_stage1: the raw bytes bound the output of the writer (with tags, the longest suffix per token).  The
     // reannotate writer's line is its raw text, a marker per character after the first, the written input tags and the
     // model's suffixes.  The written input tags of a character are at most the bytes of its tag region, and the raw text,
@@ -1628,38 +1612,30 @@ void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     // input bytes, so the same bound holds.
     const size_t out_need = 3 * nb + n + 4 + (job.tags ? nb * p.dt.max_suffix : 0);
     const bool reannotate = job.kind == kJobReannotate;
-    Scratch::ensure(s.d_out, s.out_cap, out_need);
-    PartArgs e;
+    s.out.ensure(out_need);
     e.text = ch.sp.text;
     e.offsets = ch.sp.offsets;
     e.trims = ch.sp.trims;
     e.n_sent = n;
-    e.surface = static_cast<uint8_t*>(s.d_gtext);
-    e.surf_offsets = static_cast<uint64_t*>(s.d_goff);
-    e.char_offsets = static_cast<uint64_t*>(s.d_gcoff);
-    e.given = static_cast<uint8_t*>(s.d_gbnd);
-    e.state = static_cast<uint64_t*>(s.d_tokg);
+    e.state = s.tokg.get();
     e.ticket = reinterpret_cast<uint32_t*>(e.state + ng);
-    e.err = static_cast<uint64_t*>(s.d_evtot) + kEvalTotals;
     cuda_check(cudaMemsetAsync(e.err, 0xFF, 8, st), "cudaMemset");
     cuda_check(launch_part_parse(e, st), "launch(part parse)");
     PartTagArgs pt;
     if (reannotate && job.keep_tags) {
         // every character of a line is followed by a marker or ends the line: at most (nb + 1) / 2 characters
-        Scratch::ensure(s.d_ptag, s.ptag_cap, 8 * ((nb + 1) / 2 + 2));
+        pt.regions = s.ptag.ensure(8 * ((nb + 1) / 2 + 2));
         pt.text = e.text;
         pt.offsets = e.offsets;
         pt.trims = e.trims;
         pt.n_sent = n;
         pt.char_offsets = e.char_offsets;
-        pt.regions = static_cast<uint2*>(s.d_ptag);
         cuda_check(launch_part_tags(pt, st), "launch(part tags)");
     }
     AnnArgs ann;
     if (reannotate) {
-        Scratch::ensure(s.d_pmark, s.pmark_cap, nb + 4);
         ann.margin = job.margin;
-        ann.marks = static_cast<uint8_t*>(s.d_pmark);
+        ann.marks = s.pmark.ensure(nb + 4);
     }
     BatchArgs a;
     a.text = e.surface;
@@ -1669,22 +1645,22 @@ void part_stage1(const vpt_predictor& p, Scratch& s, LineChunk& ch, const LineJo
     TokArgs t = predict_lines(p, s, ch, a, nb, job, &ra, nullptr, &e, reannotate ? &ann : nullptr);
     if (ra.tok_rule) {
         // as lines_stage1: the rules' share of the output is sized from the suffixes the chunk's tokens matched
-        cuda_check(cudaMemcpyAsync(&s.h_totals[6], s.d_trule, 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
+        cuda_check(cudaMemcpyAsync(&s.totals->rule_suffix, s.trule.get(), 8, cudaMemcpyDeviceToHost, st), "D2H(rule suffixes)");
         cuda_check(cudaStreamSynchronize(st), "sync(rules)");
-        Scratch::ensure(s.d_out, s.out_cap, out_need + size_t(s.h_totals[6]));
+        s.out.ensure(out_need + size_t(s.totals->rule_suffix));
         uint64_t seen = job.rules->max_out.load();
-        while (seen < s.out_cap && !job.rules->max_out.compare_exchange_weak(seen, s.out_cap)) {}
+        while (seen < s.out.capacity() && !job.rules->max_out.compare_exchange_weak(seen, s.out.capacity())) {}
     }
     // the look-back words of the parse are free again: the writer's come from the same scratch (its launch zeroes them)
-    t.tok_state = static_cast<uint64_t*>(s.d_tokg);
+    t.tok_state = s.tokg.get();
     t.ticket = reinterpret_cast<uint32_t*>(t.tok_state + ng);
     t.total = t.tok_state + ng + 1;
-    t.total_host = &s.h_totals[3];
-    t.out = static_cast<uint8_t*>(s.d_out);
+    t.total_host = &s.totals->out_bytes;
+    t.out = s.out.get();
     if (pt.regions) cuda_check(launch_pa_rewrite(t, ra, ann.marks, e.text, pt.regions, e.char_offsets, st), "launch(reannotate)");
     else if (reannotate) cuda_check(launch_pa_write(t, ra, ann.marks, st), "launch(annotate)");
     else cuda_check(launch_tokenize_rules(t, ra, st), "launch(tok)");
-    cuda_check(cudaMemcpyAsync(&s.h_eval[kEvalTotals], e.err, 8, cudaMemcpyDeviceToHost, st), "D2H(error key)");
+    cuda_check(cudaMemcpyAsync(&s.totals->eval[kEvalTotals], e.err, 8, cudaMemcpyDeviceToHost, st), "D2H(error key)");
     if (pipeline_trace()) ch.tr.mark(2, st);
     cuda_check(cudaEventRecord(ch.done, st), "cudaEventRecord");
 }
@@ -1805,7 +1781,7 @@ struct LineRing {
             if (line_counts) {
                 // the chunk's line count is known once its split pass is done
                 cuda_check(cudaEventSynchronize(sl.ch.split), "sync(split)");
-                if (lines_issued + s.h_totals[2] <= line_capacity) counts = line_counts;
+                if (lines_issued + s.totals->lines <= line_capacity) counts = line_counts;
                 else counts_overflow = true;
             }
             eval_stage1(p, s, sl.ch, job, counts, lines_issued);
@@ -1825,7 +1801,7 @@ struct LineRing {
         Scratch& s = *sl.lease->s;
         cuda_check(cudaEventSynchronize(sl.ch.done), "sync(lines)");
         if (job.kind == VPT_STREAM_EVALUATE) {
-            const uint64_t key = s.h_eval[kEvalTotals];
+            const uint64_t key = s.totals->eval[kEvalTotals];
             if (key != kGoldNoError) {
                 const uint64_t line = lines + (key >> 34);
                 const uint32_t kind = uint32_t(key & 7u);
@@ -1834,9 +1810,9 @@ struct LineRing {
                 throw Error(kInvalidArgument, std::string("InvalidArgumentError: tokenized_text: ") + gold_error_text(kind) +
                                                   " (line " + std::to_string(line) + ")");
             }
-            for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.h_eval[i];
+            for (int i = 0; i < kEvalTotals; ++i) tot[i] += s.totals->eval[i];
         } else if (job.kind == kJobPartial || job.kind == kJobReannotate) {
-            const uint64_t key = s.h_eval[kEvalTotals];
+            const uint64_t key = s.totals->eval[kEvalTotals];
             if (key != kGoldNoError) {
                 const uint64_t l = key >> 34;
                 const uint32_t kind = uint32_t(key & 7u);
@@ -1921,10 +1897,10 @@ int tokenize_lines_impl(const vpt_predictor* p, const uint8_t* utf8, size_t n_by
     ring.run(utf8, n_bytes, [&](LineRing::Slot& sl) {
         // the copy-out overlaps the next chunks' copy-in and kernels; the ring's final synchronisation waits for it
         Scratch& s = *sl.lease->s;
-        const uint64_t nb = s.h_totals[3];
+        const uint64_t nb = s.totals->out_bytes;
         if (total + nb > out_capacity || (nb && !out)) overflow = true;
         if (!overflow && nb) {
-            cuda_check(cudaMemcpyAsync(out + total, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
+            cuda_check(cudaMemcpyAsync(out + total, s.out.get(), nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
             cuda_check(cudaEventRecord(s.ev_out, s.stream_out), "cudaEventRecord");
         }
         if (ring.trace) sl.ch.tr.mark(3, s.stream_out);
@@ -2150,13 +2126,13 @@ struct vpt_line_stream {
         uint64_t nb = 0;
         if (ring->job.kind != VPT_STREAM_EVALUATE) {
             Scratch& s = *sl.lease->s;
-            nb = s.h_totals[3];
+            nb = s.totals->out_bytes;
             if (nb > out.cap) {
                 release(out.data);
                 out.cap = std::max(size_t(nb + nb / 4), big + big / 2);
                 out.data = alloc(out.cap);
             }
-            if (nb) cuda_check(cudaMemcpyAsync(out.data, s.d_out, nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
+            if (nb) cuda_check(cudaMemcpyAsync(out.data, s.out.get(), nb, cudaMemcpyDeviceToHost, s.stream_out), "D2H(text)");
             if (ring->trace) sl.ch.tr.mark(3, s.stream_out);
             cuda_check(cudaStreamSynchronize(s.stream_out), "sync(copy-out)");
         }
@@ -2339,11 +2315,17 @@ bool predict_single_fast(const vpt_predictor* p, const uint8_t* utf8, size_t n_b
     cuda_check(cudaSetDevice(p->device), "cudaSetDevice");
     ScratchLease lease(*p);
     Scratch& s = *lease.s;
-    if (!s.h_io) {
-        cuda_check(cudaHostAlloc(reinterpret_cast<void**>(&s.h_io), kSingleIoBytes, cudaHostAllocMapped), "cudaHostAlloc");
-        cuda_check(cudaMalloc(&s.d_io, 256), "cudaMalloc(single)");
-        cuda_check(cudaMemset(s.d_io, 0, 256), "cudaMemset(single)");
+    if (!s.d_io) {  // d_io is set last: after a first call that failed half-way, the next one allocates both again
+        uint8_t* h = nullptr;
+        cuda_check(cudaHostAlloc(reinterpret_cast<void**>(&h), kSingleIoBytes, cudaHostAllocMapped), "cudaHostAlloc");
+        s.h_io.reset(h);
+        uint8_t* d = nullptr;
+        cuda_check(cudaMalloc(&d, 256), "cudaMalloc(single)");
+        std::unique_ptr<uint8_t[], CudaFree> dev(d);
+        cuda_check(cudaMemset(d, 0, 256), "cudaMemset(single)");
+        s.d_io = std::move(dev);
     }
+    uint8_t* const io = s.h_io.get();
     // layout of the pinned block: input part first, then the outputs
     const size_t o_text = 0;                                   // text, then 64 readable bytes
     const size_t o_off = align_up(n_bytes + 64, 16);           // u64 offsets[2]
@@ -2357,14 +2339,14 @@ bool predict_single_fast(const vpt_predictor* p, const uint8_t* utf8, size_t n_b
     const size_t o_tst = o_cst + 4 * n_bytes;
     const size_t end = o_tst + 4 * n_bytes;
     if (end > kSingleIoBytes) return false;
-    memcpy(s.h_io + o_text, utf8, n_bytes);
-    memset(s.h_io + o_text + n_bytes, 0, o_off - n_bytes);
+    memcpy(io + o_text, utf8, n_bytes);
+    memset(io + o_text + n_bytes, 0, o_off - n_bytes);
     uint64_t offs[2] = {0, n_bytes};
-    memcpy(s.h_io + o_off, offs, 16);
+    memcpy(io + o_off, offs, 16);
     cudaStream_t st = s.stream;
     uint8_t* hd = nullptr;  // the device's address of the pinned block (the same value under unified addressing)
-    cuda_check(cudaHostGetDevicePointer(reinterpret_cast<void**>(&hd), s.h_io, 0), "cudaHostGetDevicePointer");
-    uint8_t* d = static_cast<uint8_t*>(s.d_io);
+    cuda_check(cudaHostGetDevicePointer(reinterpret_cast<void**>(&hd), io, 0), "cudaHostGetDevicePointer");
+    uint8_t* d = s.d_io.get();
     BatchArgs a;
     a.text = hd + o_text;
     a.offsets = reinterpret_cast<const uint64_t*>(hd + o_off);
@@ -2389,19 +2371,19 @@ bool predict_single_fast(const vpt_predictor* p, const uint8_t* utf8, size_t n_b
     cuda_check(cudaStreamSynchronize(st), "sync(single)");
     int32_t status;
     uint32_t n;
-    memcpy(&status, s.h_io + o_stat, 4);
-    memcpy(&n, s.h_io + o_stat + 4, 4);
+    memcpy(&status, io + o_stat, 4);
+    memcpy(&n, io + o_stat + 4, 4);
     if (n_chars_out) *n_chars_out = n;
     if (status != 0) throw Error(kInternal, "internal error: device validation disagrees with host validation");
     const size_t nb = n > 0 ? n - 1 : 0;
     if (nb > out_capacity || (nb && !boundaries_out) || (want_states && n > states_capacity))
         throw Error(kInvalidArgument, "InvalidArgumentError: out_capacity/states_capacity: too small for the batch");
     if (nb) {
-        memcpy(boundaries_out, s.h_io + o_bnd, nb);
-        if (scores_out) memcpy(scores_out, s.h_io + o_sc, 4 * nb);
+        memcpy(boundaries_out, io + o_bnd, nb);
+        if (scores_out) memcpy(scores_out, io + o_sc, 4 * nb);
     }
-    if (char_states_out) memcpy(char_states_out, s.h_io + o_cst, 4 * size_t(n));
-    if (type_states_out) memcpy(type_states_out, s.h_io + o_tst, 4 * size_t(n));
+    if (char_states_out) memcpy(char_states_out, io + o_cst, 4 * size_t(n));
+    if (type_states_out) memcpy(type_states_out, io + o_tst, 4 * size_t(n));
     return true;
 }
 
@@ -2561,45 +2543,38 @@ int vpt_predict_batch_tags(const vpt_predictor* p, const uint8_t* utf8, const ui
     const size_t shift = size_t(byte_lo & 15);
     const WorkspaceLayout wl = workspace_layout(n_sent);
     const size_t nt = p->n_tags;
-    Scratch::ensure(s.d_text, s.text_cap, shift + nbytes + 64);
-    Scratch::ensure(s.d_off, s.off_cap, 8 * (n_sent + 1));
-    Scratch::ensure(s.d_ws, s.ws_cap, wl.total);
-    Scratch::ensure(s.d_status, s.status_cap, 4 * n_sent);
-    Scratch::ensure(s.d_boff, s.boff_cap, 8 * (n_sent + 1));
-    Scratch::ensure(s.d_coff, s.coff_cap, 8 * (n_sent + 1));
-    Scratch::ensure(s.d_scores, s.scores_cap, 4 * nbytes + 16);      // a character has at least one byte
-    Scratch::ensure(s.d_bounds, s.bounds_cap, nbytes + 16);
-    Scratch::ensure(s.d_cst, s.cst_cap, 4 * nbytes + 16);
-    Scratch::ensure(s.d_tst, s.tst_cap, 4 * nbytes + 16);
-    Scratch::ensure(s.d_tok, s.tok_cap, 4 * nbytes + 16);
-    Scratch::ensure(s.d_cand, s.cand_cap, 4 * nbytes * nt + 16);
-    if (nbytes)
-        cuda_check(cudaMemcpyAsync(static_cast<uint8_t*>(s.d_text) + shift, utf8 + byte_lo, nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
-    cuda_check(cudaMemcpyAsync(s.d_off, byte_offsets, 8 * (n_sent + 1), cudaMemcpyHostToDevice, st), "H2D(offsets)");
     BatchArgs a;
-    a.text = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(s.d_text) + shift - uintptr_t(byte_lo));
-    a.offsets = static_cast<const uint64_t*>(s.d_off);
+    uint8_t* const text = s.text.ensure(shift + nbytes + 64);
+    uint64_t* const offsets = s.off.ensure(8 * (n_sent + 1));
+    bind_workspace(a, s.ws.ensure(wl.total), n_sent);
+    a.status = s.status.ensure(4 * n_sent);
+    a.bound_offsets = s.boff.ensure(8 * (n_sent + 1));
+    a.char_offsets = s.coff.ensure(8 * (n_sent + 1));
+    a.scores = s.scores.ensure(4 * nbytes + 16);      // a character has at least one byte
+    a.boundaries = s.bounds.ensure(nbytes + 16);
+    a.char_states = s.cst.ensure(4 * nbytes + 16);
+    a.type_states = s.tst.ensure(4 * nbytes + 16);
+    int32_t* const tag_token = s.tok.ensure(4 * nbytes + 16);
+    // the i32 candidates of every character, in the buffer that holds the u8 candidates of token records elsewhere
+    int32_t* const tag_cand = reinterpret_cast<int32_t*>(s.cand.ensure(4 * nbytes * nt + 16));
+    if (nbytes)
+        cuda_check(cudaMemcpyAsync(text + shift, utf8 + byte_lo, nbytes, cudaMemcpyHostToDevice, st), "H2D(text)");
+    cuda_check(cudaMemcpyAsync(offsets, byte_offsets, 8 * (n_sent + 1), cudaMemcpyHostToDevice, st), "H2D(offsets)");
+    a.text = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(text) + shift - uintptr_t(byte_lo));
+    a.offsets = offsets;
     a.n_sent = n_sent;
-    bind_workspace(a, s.d_ws, n_sent);
-    a.status = static_cast<int32_t*>(s.d_status);
-    a.bound_offsets = static_cast<uint64_t*>(s.d_boff);
-    a.char_offsets = static_cast<uint64_t*>(s.d_coff);
-    a.scores = static_cast<int32_t*>(s.d_scores);
-    a.boundaries = static_cast<uint8_t*>(s.d_bounds);
-    a.char_states = static_cast<uint32_t*>(s.d_cst);
-    a.type_states = static_cast<uint32_t*>(s.d_tst);
-    a.totals_host = &s.h_totals[0];
-    s.h_totals[2] = 0;
+    a.totals_host = s.totals->bounds_chars;
     cuda_check(launch_batch(p->dm, a, st), "launch(batch)");
-    uint32_t* d_unserved = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(s.d_ws) + wl.ticket + 128);
+    // a word behind the ticket in the workspace's 256-byte ticket slot
+    uint32_t* d_unserved = reinterpret_cast<uint32_t*>(s.ws.get() + wl.ticket + 128);
     cuda_check(cudaMemsetAsync(d_unserved, 0, 4, st), "memset");
     TagArgs t = tag_args(p->dt, a);
-    t.tag_token = static_cast<int32_t*>(s.d_tok);
-    t.tag_cand = static_cast<int32_t*>(s.d_cand);
+    t.tag_token = tag_token;
+    t.tag_cand = tag_cand;
     t.n_unserved = d_unserved;
     cuda_check(launch_tags(p->dt, t, st), "launch(tags)");
     cuda_check(cudaStreamSynchronize(st), "sync(tags)");  // the totals are in pinned host memory now
-    const uint64_t nb = s.h_totals[0], nc = s.h_totals[1];
+    const uint64_t nb = s.totals->bounds_chars[0], nc = s.totals->bounds_chars[1];
     if (n_boundaries_out) *n_boundaries_out = nb;
     if (n_chars_out) *n_chars_out = nc;
     if (nb > out_capacity || nc > chars_capacity)
@@ -2607,15 +2582,15 @@ int vpt_predict_batch_tags(const vpt_predictor* p, const uint8_t* utf8, const ui
     uint32_t unserved = 0;
     cuda_check(cudaMemcpyAsync(&unserved, d_unserved, 4, cudaMemcpyDeviceToHost, st), "D2H");
     if (nb) {
-        if (scores_out) cuda_check(cudaMemcpyAsync(scores_out, s.d_scores, 4 * nb, cudaMemcpyDeviceToHost, st), "D2H(scores)");
-        cuda_check(cudaMemcpyAsync(boundaries_out, s.d_bounds, nb, cudaMemcpyDeviceToHost, st), "D2H(boundaries)");
+        if (scores_out) cuda_check(cudaMemcpyAsync(scores_out, a.scores, 4 * nb, cudaMemcpyDeviceToHost, st), "D2H(scores)");
+        cuda_check(cudaMemcpyAsync(boundaries_out, a.boundaries, nb, cudaMemcpyDeviceToHost, st), "D2H(boundaries)");
     }
-    cuda_check(cudaMemcpyAsync(bound_offsets_out, s.d_boff, 8 * (n_sent + 1), cudaMemcpyDeviceToHost, st), "D2H(offsets)");
-    cuda_check(cudaMemcpyAsync(char_offsets_out, s.d_coff, 8 * (n_sent + 1), cudaMemcpyDeviceToHost, st), "D2H(offsets)");
-    if (status_out) cuda_check(cudaMemcpyAsync(status_out, s.d_status, 4 * n_sent, cudaMemcpyDeviceToHost, st), "D2H(status)");
+    cuda_check(cudaMemcpyAsync(bound_offsets_out, a.bound_offsets, 8 * (n_sent + 1), cudaMemcpyDeviceToHost, st), "D2H(offsets)");
+    cuda_check(cudaMemcpyAsync(char_offsets_out, a.char_offsets, 8 * (n_sent + 1), cudaMemcpyDeviceToHost, st), "D2H(offsets)");
+    if (status_out) cuda_check(cudaMemcpyAsync(status_out, a.status, 4 * n_sent, cudaMemcpyDeviceToHost, st), "D2H(status)");
     if (nc) {
-        cuda_check(cudaMemcpyAsync(tag_token_out, s.d_tok, 4 * nc, cudaMemcpyDeviceToHost, st), "D2H(tags)");
-        cuda_check(cudaMemcpyAsync(tag_cand_out, s.d_cand, 4 * nc * nt, cudaMemcpyDeviceToHost, st), "D2H(tags)");
+        cuda_check(cudaMemcpyAsync(tag_token_out, tag_token, 4 * nc, cudaMemcpyDeviceToHost, st), "D2H(tags)");
+        cuda_check(cudaMemcpyAsync(tag_cand_out, tag_cand, 4 * nc * nt, cudaMemcpyDeviceToHost, st), "D2H(tags)");
     }
     cuda_check(cudaStreamSynchronize(st), "sync(copy-out)");
     if (n_unserved_out) *n_unserved_out = unserved;
@@ -2633,17 +2608,14 @@ size_t device_score_len_bound(const vpt_predictor* p) {
     return std::min<size_t>(m, size_t(kTagMaxScores));
 }
 
-// Scratch of the tag candidate scores of one chunk of at most `nc` token records; its total arrives in h_totals[7].
+// Scratch of the tag candidate scores of one chunk of at most `nc` token records; its total arrives in `tag_scores`.
 TagScoreArgs bind_tag_scores(Scratch& s, uint64_t nc, size_t len_bound) {
-    Scratch::ensure(s.d_scoff, s.scoff_cap, 4 * nc + 16);
-    Scratch::ensure(s.d_scblk, s.scblk_cap, 8 * (nc / kScoreScanBlock + 4));
-    Scratch::ensure(s.d_tagsc, s.tagsc_cap, 4 * nc * len_bound + 16);
     TagScoreArgs sc;
-    sc.rec_off = static_cast<uint32_t*>(s.d_scoff);
-    sc.blk = static_cast<uint64_t*>(s.d_scblk);
-    sc.scores = static_cast<int32_t*>(s.d_tagsc);
-    s.h_totals[7] = 0;
-    sc.total_host = &s.h_totals[7];
+    sc.rec_off = s.scoff.ensure(4 * nc + 16);
+    sc.blk = s.scblk.ensure(8 * (nc / kScoreScanBlock + 4));
+    sc.scores = s.tagsc.ensure(4 * nc * len_bound + 16);
+    s.totals->tag_scores = 0;
+    sc.total_host = &s.totals->tag_scores;
     return sc;
 }
 
@@ -2704,13 +2676,16 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
     bool overflow = false;
     // pinned words that receive every chunk's first bit word (merged into the output at the end)
     Scratch& s0 = ring.scratch(0);
-    if (s0.side_cap < nchunks) {
-        if (s0.h_side) { cudaFreeHost(s0.h_side); s0.h_side = nullptr; s0.side_cap = 0; }
+    if (s0.side_words < nchunks) {
+        s0.h_side.reset();
+        s0.side_words = 0;
         const size_t want = std::max<size_t>(256, 2 * nchunks);
-        cuda_check(cudaMallocHost(reinterpret_cast<void**>(&s0.h_side), 4 * want), "cudaMallocHost");
-        s0.side_cap = want;
+        uint32_t* q = nullptr;
+        cuda_check(cudaMallocHost(reinterpret_cast<void**>(&q), 4 * want), "cudaMallocHost");
+        s0.h_side.reset(q);
+        s0.side_words = want;
     }
-    uint32_t* const h_side = s0.h_side;
+    uint32_t* const h_side = s0.h_side.get();
     std::vector<uint32_t> h_unserved(nchunks, 0);
     std::vector<uint64_t> nb_base(nchunks, 0);  // the chunk's first boundary in the batch
     std::vector<char> copied(nchunks, 0);       // the chunk's first bit word is in h_side
@@ -2721,18 +2696,12 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
         nb_total += ch.nb;
         if ((nb_total + 31) / 32 > bits_capacity_words || (nb_total && !boundary_bits_out)) { overflow = true; return false; }
         BatchArgs& a = ch.a;
-        Scratch::ensure(s.d_bounds, s.bounds_cap, ch.nb + 4);
+        a.boundaries = s.bounds.ensure(ch.nb + 4);
         a.scores = nullptr;
-        if (!scores_optional(p->dm)) {
-            Scratch::ensure(s.d_scores, s.scores_cap, 4 * ch.nb + 4);
-            a.scores = static_cast<int32_t*>(s.d_scores);
-        }
-        a.boundaries = static_cast<uint8_t*>(s.d_bounds);
+        if (!scores_optional(p->dm)) a.scores = s.scores.ensure(4 * ch.nb + 4);
         if (want_tags) {
-            Scratch::ensure(s.d_cst, s.cst_cap, 4 * ch.nc + 4);
-            Scratch::ensure(s.d_tst, s.tst_cap, 4 * ch.nc + 4);
-            a.char_states = static_cast<uint32_t*>(s.d_cst);
-            a.type_states = static_cast<uint32_t*>(s.d_tst);
+            a.char_states = s.cst.ensure(4 * ch.nc + 4);
+            a.type_states = s.tst.ensure(4 * ch.nc + 4);
         }
         // (chunk-local offsets: bound_base / char_base stay 0)
         if (pipeline_trace()) ch.tr.mark(1, st);
@@ -2746,18 +2715,17 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
         k.n_bound = ch.nb;
         k.bit_base = uint32_t(nb_base[c] & 31);
         const size_t nwords = size_t((k.bit_base + ch.nb + 31) / 32);
-        Scratch::ensure(s.d_bits, s.bits_cap, 4 * nwords + 16);
-        Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
-        k.bits = static_cast<uint32_t*>(s.d_bits);
-        k.status8 = static_cast<uint8_t*>(s.d_st8);
+        k.bits = s.bits.ensure(4 * nwords + 16);
+        k.status8 = s.st8.ensure(ch.n + 16);
         if (want_tokens) {
             bind_token_counts(s, k, ch.n);
-            k.tok_total_host = &s.h_totals[4];
+            k.tok_total_host = &s.totals->tokens;
         }
-        s.h_totals[4] = 0;
+        s.totals->tokens = 0;
         cuda_check(launch_compact(k, st), "launch(compact)");
         if (want_tags) {
-            uint32_t* d_unserved = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(s.d_ws) + workspace_layout(ch.n).ticket + 128);
+            // a word behind the ticket in the workspace's 256-byte ticket slot
+            uint32_t* d_unserved = reinterpret_cast<uint32_t*>(s.ws.get() + workspace_layout(ch.n).ticket + 128);
             cuda_check(cudaMemsetAsync(d_unserved, 0, 4, st), "memset");
             TagArgs t = tag_args(p->dt, a);
             t.n_unserved = d_unserved;
@@ -2774,8 +2742,8 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
         return true;
     };
     auto copy_out = [&](size_t c, ChunkState& ch, Scratch& s, cudaStream_t so) {
-        const uint64_t ntok = want_tokens ? s.h_totals[4] : 0;
-        const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
+        const uint64_t ntok = want_tokens ? s.totals->tokens : 0;
+        const uint64_t nsc = want_scores ? s.totals->tag_scores : 0;
         if (want_tags && tok_total + ntok > token_capacity) overflow = true;
         if (score_total + nsc > score_capacity) overflow = true;
         if (!overflow) {
@@ -2786,20 +2754,20 @@ int vpt_predict_batch_compact_tag_scores(const vpt_predictor* p, const uint8_t* 
                 // the chunk's first word may share its low bits with the previous chunk: it comes back through a pinned
                 // word and is merged on the host at the end; the other words go straight to their place
                 if (bit_base == 0) boundary_bits_out[w0] = 0;
-                cuda_check(cudaMemcpyAsync(&h_side[c], s.d_bits, 4, cudaMemcpyDeviceToHost, so), "D2H(bits)");
+                cuda_check(cudaMemcpyAsync(&h_side[c], s.bits.get(), 4, cudaMemcpyDeviceToHost, so), "D2H(bits)");
                 if (nwords > 1)
-                    cuda_check(cudaMemcpyAsync(boundary_bits_out + w0 + 1, static_cast<uint32_t*>(s.d_bits) + 1, 4 * (nwords - 1),
+                    cuda_check(cudaMemcpyAsync(boundary_bits_out + w0 + 1, s.bits.get() + 1, 4 * (nwords - 1),
                                                cudaMemcpyDeviceToHost, so), "D2H(bits)");
             }
             cuda_check(cudaMemcpyAsync(n_chars_out + ch.s_lo, ch.a.n_chars, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_chars)");
-            cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_st8, ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
-            if (n_tokens_out) cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.d_ntok, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
+            cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.st8.get(), ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
+            if (n_tokens_out) cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.ntok.get(), 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
             if (want_tags && ntok) {
-                cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.d_tok, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
-                if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.d_cand, ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.tok.get(), 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.cand.get(), ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
             }
             if (nsc)
-                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
+                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.tagsc.get(), 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
             copied[c] = ch.nb != 0;
         }
         tok_total += ntok;
@@ -2964,27 +2932,19 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
         cudaStream_t st = s.stream;
         const uint64_t nb = ch.nb, nc = ch.nc;
         BatchArgs& a = ch.a;
-        Scratch::ensure(s.d_bounds, s.bounds_cap, nb + 4);
+        a.boundaries = s.bounds.ensure(nb + 4);
         a.scores = nullptr;
-        if (!scores_optional(dm)) {
-            Scratch::ensure(s.d_scores, s.scores_cap, 4 * nb + 4);
-            a.scores = static_cast<int32_t*>(s.d_scores);
-        }
-        a.boundaries = static_cast<uint8_t*>(s.d_bounds);
+        if (!scores_optional(dm)) a.scores = s.scores.ensure(4 * nb + 4);
         if (tags) {
-            Scratch::ensure(s.d_cst, s.cst_cap, 4 * nc + 4);
-            Scratch::ensure(s.d_tst, s.tst_cap, 4 * nc + 4);
-            a.char_states = static_cast<uint32_t*>(s.d_cst);
-            a.type_states = static_cast<uint32_t*>(s.d_tst);
+            a.char_states = s.cst.ensure(4 * nc + 4);
+            a.type_states = s.tst.ensure(4 * nc + 4);
         }
-        Scratch::ensure(s.d_st8, s.st8_cap, ch.n + 16);
-        Scratch::ensure(s.d_ends, s.ends_cap, 4 * nc + 16);  // a token has at least one character
         SpanStage b;
-        b.status8 = static_cast<uint8_t*>(s.d_st8);
+        b.status8 = s.st8.ensure(ch.n + 16);
+        b.token_ends = s.ends.ensure(4 * nc + 16);  // a token has at least one character
         bind_token_counts(s, b, ch.n);
-        b.tok_total_host = &s.h_totals[4];
-        s.h_totals[4] = 0;
-        b.token_ends = static_cast<uint32_t*>(s.d_ends);
+        b.tok_total_host = &s.totals->tokens;
+        s.totals->tokens = 0;
         TagScoreArgs sc;
         if (tags) {
             bind_token_records(*p, s, b, nc);
@@ -3001,22 +2961,22 @@ int vpt_token_spans_tag_scores(const vpt_predictor* p, const uint8_t* utf8, cons
         return true;
     };
     auto copy_out = [&](size_t, ChunkState& ch, Scratch& s, cudaStream_t so) {
-        const uint64_t ntok = s.h_totals[4];
-        const uint64_t nsc = want_scores ? s.h_totals[7] : 0;
+        const uint64_t ntok = s.totals->tokens;
+        const uint64_t nsc = want_scores ? s.totals->tag_scores : 0;
         if (tok_total + ntok > token_capacity || (ntok && !token_ends_out)) overflow = true;
         if (score_total + nsc > score_capacity) overflow = true;
         if (!overflow) {
-            cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.d_ntok, 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
-            cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.d_st8, ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
+            cuda_check(cudaMemcpyAsync(n_tokens_out + ch.s_lo, s.ntok.get(), 4 * ch.n, cudaMemcpyDeviceToHost, so), "D2H(n_tokens)");
+            cuda_check(cudaMemcpyAsync(status_out + ch.s_lo, s.st8.get(), ch.n, cudaMemcpyDeviceToHost, so), "D2H(status)");
             if (ntok) {
-                cuda_check(cudaMemcpyAsync(token_ends_out + tok_total, s.d_ends, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(ends)");
+                cuda_check(cudaMemcpyAsync(token_ends_out + tok_total, s.ends.get(), 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(ends)");
                 if (tags) {
-                    cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.d_tok, 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
-                    if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.d_cand, ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                    cuda_check(cudaMemcpyAsync(token_ids_out + tok_total, s.tok.get(), 4 * ntok, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
+                    if (nt) cuda_check(cudaMemcpyAsync(token_cands_out + tok_total * nt, s.cand.get(), ntok * nt, cudaMemcpyDeviceToHost, so), "D2H(tokens)");
                 }
             }
             if (nsc)
-                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.d_tagsc, 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
+                cuda_check(cudaMemcpyAsync(tag_scores_out + score_total, s.tagsc.get(), 4 * nsc, cudaMemcpyDeviceToHost, so), "D2H(tag scores)");
         }
         tok_total += ntok;
         score_total += nsc;
